@@ -58,6 +58,13 @@ class GsbVolumeDesc(C.Structure):
     ]
 
 
+class GsbPointGrid(C.Structure):
+    _fields_ = [
+        ("origin", C.c_double * 3), ("cell", C.c_double), ("dims", C.c_int32 * 3), ("points", _vp), ("n_points", C.c_int64),
+        ("cell_start", _vp), ("ids", _vp),
+    ]
+
+
 # name -> (restype, argtypes); every symbol include/gs2mesh_b200.h declares
 SIGNATURES = {
     "gsb_last_error": (C.c_char_p, []),
@@ -96,6 +103,12 @@ SIGNATURES = {
     "gsb_mesh_emit": (C.c_int, [_vp, C.POINTER(C.c_int32), _vp, C.c_uint32, _vp, _vp, _vp]),
     "gsb_mesh_vertices": (C.c_int, [_vp, C.POINTER(C.c_int32), _vp, C.c_int64, _vp, _vp, _vp]),
     "gsb_mesh_vertex_normals": (C.c_int, [_vp, C.c_int64, _vp, C.c_int64, _vp, _vp]),
+    "gsb_eval_sample_count": (C.c_int, [_vp, C.c_int64, _vp, C.c_int64, C.c_double, _vp, _vp]),
+    "gsb_eval_sample_emit": (C.c_int, [_vp, C.c_int64, _vp, C.c_int64, C.c_double, _vp, _vp, _vp]),
+    "gsb_eval_grid_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int64]),
+    "gsb_eval_grid_build": (C.c_int, [C.POINTER(GsbPointGrid), _vp, C.c_size_t, _vp]),
+    "gsb_eval_nearest": (C.c_int, [C.POINTER(GsbPointGrid), _vp, C.c_int64, C.c_double, _vp, _vp, _vp]),
+    "gsb_eval_radius_downsample": (C.c_int, [C.POINTER(GsbPointGrid), C.c_double, _vp, _vp, _vp, C.POINTER(C.c_int32), _vp]),
 }
 
 _lib = None

@@ -152,11 +152,13 @@ _PLY_TYPES = {"float": "<f4", "float32": "<f4", "double": "<f8", "float64": "<f8
               "int32": "<i4", "uint": "<u4", "uint32": "<u4", "short": "<i2", "ushort": "<u2", "char": "i1"}
 
 
-def _read_vertex_table(path):
+def _read_vertex_table(path, with_faces=False):
+    """The vertex element of a binary-little-endian or ascii PLY as a structured array; with_faces also returns the face
+    element's triangles (int64 [M,3], from a `property list <uchar|int> <int|uint>` of length 3), or None without one."""
     with open(path, "rb") as f:
         if f.readline().strip() != b"ply":
             raise ValueError(f"{path}: not a PLY file")
-        fmt, count, props, in_vertex = None, 0, [], False
+        fmt, elements = None, []  # [name, count, props]; props of a list property: ("list", count type, index type)
         while True:
             line = f.readline()
             if not line:
@@ -167,24 +169,80 @@ def _read_vertex_table(path):
             if tok[0] == "format":
                 fmt = tok[1]
             elif tok[0] == "element":
-                in_vertex = tok[1] == "vertex"
-                if in_vertex:
-                    count = int(tok[2])
-            elif tok[0] == "property" and in_vertex:
+                elements.append([tok[1], int(tok[2]), []])
+            elif tok[0] == "property" and elements:
                 if tok[1] == "list":
-                    raise ValueError(f"{path}: list property on the vertex element is not supported")
-                props.append((tok[2], _PLY_TYPES[tok[1]]))
+                    if elements[-1][0] == "vertex":
+                        raise ValueError(f"{path}: list property on the vertex element is not supported")
+                    elements[-1][2].append(("list", _PLY_TYPES[tok[2]], _PLY_TYPES[tok[3]]))
+                else:
+                    elements[-1][2].append((tok[2], _PLY_TYPES[tok[1]]))
             elif tok[0] == "end_header":
                 break
+        if not elements or elements[0][0] != "vertex":
+            raise ValueError(f"{path}: the first PLY element must be 'vertex'")
+        _, count, props = elements[0]
+        face = elements[1] if len(elements) > 1 and elements[1][0] == "face" else None
+        if face is not None and (len(face[2]) != 1 or face[2][0][0] != "list"):
+            raise ValueError(f"{path}: the face element must hold exactly one list property")
         if fmt == "binary_little_endian":
-            return np.fromfile(f, dtype=np.dtype(props), count=count)
-        if fmt == "ascii":
-            raw = np.loadtxt(f, max_rows=count, ndmin=2)
-            out = np.zeros(count, dtype=np.dtype(props))
+            vert = np.fromfile(f, dtype=np.dtype(props), count=count)
+            tris = None
+            if face is not None:
+                _, ct, it = face[2][0]
+                rec = np.fromfile(f, dtype=np.dtype([("n", ct), ("v", it, (3,))]), count=face[1])
+                if len(rec) != face[1] or (rec["n"] != 3).any():
+                    raise ValueError(f"{path}: only triangle faces are supported")
+                tris = rec["v"].astype(np.int64)
+        elif fmt == "ascii":
+            lines = [ln for ln in f.read().decode("ascii").splitlines() if ln.strip()]
+            raw = np.array([ln.split() for ln in lines[:count]], dtype=np.float64).reshape(count, len(props))
+            vert = np.zeros(count, dtype=np.dtype(props))
             for j, (name, _) in enumerate(props):
-                out[name] = raw[:, j]
-            return out
-        raise ValueError(f"{path}: unsupported PLY format {fmt}")
+                vert[name] = raw[:, j]
+            tris = None
+            if face is not None:
+                rows = [ln.split() for ln in lines[count:count + face[1]]]
+                if len(rows) != face[1] or any(len(r) != 4 or r[0] != "3" for r in rows):
+                    raise ValueError(f"{path}: only triangle faces are supported")
+                tris = np.array([r[1:] for r in rows], dtype=np.int64).reshape(-1, 3)
+        else:
+            raise ValueError(f"{path}: unsupported PLY format {fmt}")
+        return (vert, tris) if with_faces else vert
+
+
+def read_point_cloud_ply(path):
+    """o3d.io.read_point_cloud(path).points (eval.py:76-77, 114-115): float64 [N,3]."""
+    v = _read_vertex_table(path)
+    return np.stack([v["x"], v["y"], v["z"]], axis=1).astype(np.float64)
+
+
+def read_triangle_mesh_ply(path):
+    """o3d.io.read_triangle_mesh(path) vertices / triangles (eval.py:46-49): (float64 [N,3], int64 [M,3])."""
+    v, tris = _read_vertex_table(path, with_faces=True)
+    xyz = np.stack([v["x"], v["y"], v["z"]], axis=1).astype(np.float64)
+    return xyz, (np.zeros((0, 3), np.int64) if tris is None else tris)
+
+
+def write_point_cloud_ply(path, points, colors=None):
+    """o3d.io.write_point_cloud for eval.py's visualisation clouds (eval.py:21-25): binary little-endian, double xyz,
+    uchar rgb = round(255 * colour)."""
+    points = np.asarray(points, dtype=np.float64).reshape(-1, 3)
+    props = [("x", "<f8"), ("y", "<f8"), ("z", "<f8")]
+    header = ["ply", "format binary_little_endian 1.0", f"element vertex {len(points)}", "property double x",
+              "property double y", "property double z"]
+    if colors is not None:
+        props += [("red", "u1"), ("green", "u1"), ("blue", "u1")]
+        header += ["property uchar red", "property uchar green", "property uchar blue"]
+    tab = np.zeros(len(points), dtype=props)
+    tab["x"], tab["y"], tab["z"] = points.T
+    if colors is not None:
+        rgb = np.clip(np.rint(np.asarray(colors, dtype=np.float64).reshape(-1, 3) * 255.0), 0, 255).astype(np.uint8)
+        tab["red"], tab["green"], tab["blue"] = rgb.T
+    with open(path, "wb") as f:
+        f.write(("\n".join(header + ["end_header"]) + "\n").encode("ascii"))
+        f.write(tab.tobytes())
+    return path
 
 
 def read_gaussian_ply(path, sh_degree=3) -> GaussianCloud:

@@ -318,6 +318,49 @@ int gsb_mesh_vertices(const GsbVolume* vol, const int32_t* window, const int64_t
 int gsb_mesh_vertex_normals(const double* xyz, int64_t n_vertices, const int64_t* triangles, int64_t n_triangles, double* normals,
                             void* stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Mesh-quality evaluation (evaluation/DTU/eval_code/eval.py, MobileBrick evaluate.py) without Open3D / sklearn.
+ * All arithmetic is fp64 with explicit roundings (no FMA contraction), in the reference's operation order.
+ * ------------------------------------------------------------------------------------------
+ * Surface sampling (eval.py:48-71), two passes:
+ *   gsb_eval_sample_count  tri_counts[t] = points triangle t contributes (0 for zero-area triangles)
+ *   gsb_eval_sample_emit   writes them (fp64 xyz) at samples + 3*tri_offsets[t], in np.mgrid order
+ * vertices: device double [n_vertices,3]; triangles: device int64 [n_triangles,3]; thresh = downsample_density. */
+int gsb_eval_sample_count(const double* vertices, int64_t n_vertices, const int64_t* triangles, int64_t n_triangles, double thresh,
+                          int64_t* tri_counts, void* stream);
+int gsb_eval_sample_emit(const double* vertices, int64_t n_vertices, const int64_t* triangles, int64_t n_triangles, double thresh,
+                         const int64_t* tri_offsets, double* samples, void* stream);
+
+/* Uniform grid over reference points: point ids counting-sorted by cell (x-major, cell index (cx*dims[1]+cy)*dims[2]+cz,
+ * cx = floor((x - origin[0]) / cell)).  origin / dims must cover every point: a point outside would be clamped into a
+ * border cell, and the searches below are only exact when each point lies in its cell. */
+typedef struct GsbPointGrid {
+  double origin[3];
+  double cell;              /* cell edge length, > 0                                   */
+  int32_t dims[3];          /* cells per axis; dims[0]*dims[1]*dims[2] < 2^31           */
+  const double* points;     /* device double [n_points,3]                             */
+  int64_t n_points;
+  int64_t* cell_start;      /* device int64 [cells+1]: ids of cell c are ids[cell_start[c] .. cell_start[c+1]) */
+  int64_t* ids;             /* device int64 [n_points]                                */
+} GsbPointGrid;
+
+size_t gsb_eval_grid_workspace_bytes(int64_t n_points, int64_t n_cells);
+/* Fills grid->cell_start and grid->ids (order inside a cell is unspecified). */
+int gsb_eval_grid_build(const GsbPointGrid* grid, void* workspace, size_t workspace_bytes, void* stream);
+/* Exact 1-nearest neighbour of every query among the grid's points: dist = sqrt(((dx*dx)+dy*dy)+dz*dz) (sklearn's kd_tree
+ * kneighbors distance, bit for bit), index = the nearest point (lowest index among equal squared distances).  Queries
+ * with no point closer than max_dist get dist = +inf, index = -1, and the search stops there; max_dist = +inf searches
+ * until the nearest point is found. */
+int gsb_eval_nearest(const GsbPointGrid* grid, const double* queries, int64_t n_queries, double max_dist, double* dist,
+                     int64_t* index, void* stream);
+/* Greedy radius downsampling of the grid's points in index order (eval.py:88-93): keep[p] = 1 iff no earlier kept point q
+ * has ((dx*dx)+dy*dy)+dz*dz <= radius*radius (sklearn radius_neighbors, inclusive).  Needs grid->cell > radius.
+ * Runs rounds of the parallel greedy rule and reads the undecided count every 4 rounds: SYNCHRONISES the stream.
+ * keep: device uint8[n_points]; counters: device uint32[4] scratch; host_undecided: pinned host uint32[1];
+ * rounds (may be NULL) receives the number of rounds run. */
+int gsb_eval_radius_downsample(const GsbPointGrid* grid, double radius, uint8_t* keep, uint32_t* counters,
+                               uint32_t* host_undecided, int32_t* rounds, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
