@@ -109,6 +109,9 @@ SIGNATURES = {
     "gsb_eval_grid_build": (C.c_int, [C.POINTER(GsbPointGrid), _vp, C.c_size_t, _vp]),
     "gsb_eval_nearest": (C.c_int, [C.POINTER(GsbPointGrid), _vp, C.c_int64, C.c_double, _vp, _vp, _vp]),
     "gsb_eval_radius_downsample": (C.c_int, [C.POINTER(GsbPointGrid), C.c_double, _vp, _vp, _vp, C.POINTER(C.c_int32), _vp]),
+    "gsb_eval_mask_dilate_disk": (C.c_int, [_vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _vp, _vp, _vp]),
+    "gsb_eval_cull_vertices_by_masks": (C.c_int, [_vp, C.c_int64, _vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                                  _vp, _vp, _vp]),
 }
 
 _lib = None

@@ -12,7 +12,7 @@ PKG_DIR = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(PKG_DIR)
 CSRC = os.path.join(PKG_DIR, "csrc")
 LIB_PATH = os.path.join(PKG_DIR, "libgs2mesh_b200.so")
-SOURCES = ["gsb_raster.cu", "gsb_tsdf.cu", "gsb_mesh.cu", "gsb_reduce.cu", "gsb_eval.cu"]
+SOURCES = ["gsb_raster.cu", "gsb_tsdf.cu", "gsb_mesh.cu", "gsb_reduce.cu", "gsb_eval.cu", "gsb_cull.cu"]
 NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
               "-Xcompiler", "-fPIC", "-shared", "-I", os.path.join(ROOT, "include"), "-I", CSRC, "-ldl"]
 

@@ -361,6 +361,21 @@ int gsb_eval_nearest(const GsbPointGrid* grid, const double* queries, int64_t n_
 int gsb_eval_radius_downsample(const GsbPointGrid* grid, double radius, uint8_t* keep, uint32_t* counters,
                                uint32_t* host_undecided, int32_t* rounds, void* stream);
 
+/* Mesh culling by object masks (evaluation/DTU/eval_code/evaluate_single_scene.py:21-116, `cull_scan`).
+ * Binary dilation of n_views masks (device uint8 [n_views,height,width], nonzero = set) by the disk x*x + y*y <= r*r
+ * (skimage disk(r)); pixels outside the image are unset.  packed: device uint32 [n_views][height][(width+31)/32], pixel x
+ * of a row is bit x%32 of word x/32.  workspace: device uint8 [n_views*height*width].  0 <= radius <= 254. */
+int gsb_eval_mask_dilate_disk(const uint8_t* masks, int32_t n_views, int32_t height, int32_t width, int32_t radius,
+                              uint32_t* packed, uint8_t* workspace, void* stream);
+/* keep[i] = 0 iff some view projects vertex i (device double [n_vertices,3], rounded to fp32) strictly inside the
+ * image_width x image_height frame onto an unset pixel of its packed mask (mask_width x mask_height, the layout of
+ * gsb_eval_mask_dilate_disk), else 1.  matrices: device float [n_views][4][4], row-major, camera = M @ (x, y, z, 1).
+ * fp32 arithmetic in the reference's torch order on the GPU (DESIGN.md section 7a); no test of depth > 0, and a
+ * non-finite projection is never culled. */
+int gsb_eval_cull_vertices_by_masks(const double* vertices, int64_t n_vertices, const float* matrices, int32_t n_views,
+                                    int32_t image_width, int32_t image_height, int32_t mask_width, int32_t mask_height,
+                                    const uint32_t* packed_masks, uint8_t* keep, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
