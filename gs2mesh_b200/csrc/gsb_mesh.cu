@@ -114,9 +114,12 @@ __global__ void __launch_bounds__(256) mc_brick_kernel(const VolView v, const ui
   if (mode == 0 && threadIdx.x == 0) tri_counts[blockIdx.x] = s_count;
 }
 
-// One unique edge -> vertex position (fp64, Open3D's formula) and colour.
+// One unique edge -> vertex position and colour, fp64 with one rounding per operation in Open3D's order (no FMA
+// contraction, no reciprocal), so both equal Open3D's doubles bit for bit:
+//   pt(k) = half_voxel_length + voxel_length * index(k);  pt(axis) += f0 * voxel_length / (f0 + f1)
+//   colour = (f1 * c0 + f0 * c1) / (f0 + f1),  c = voxel colour / 255.0
 __global__ void __launch_bounds__(256) mc_vertices_kernel(const VolView v, const long long* __restrict__ keys, long long n,
-                                                          double* __restrict__ xyz, float* __restrict__ rgb) {
+                                                          double* __restrict__ xyz, double* __restrict__ rgb) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const long long NY = (long long)v.nb[1] * GSB_BRICK, NZ = (long long)v.nb[2] * GSB_BRICK;
@@ -130,11 +133,12 @@ __global__ void __launch_bounds__(256) mc_vertices_kernel(const VolView v, const
   const int dx = axis == 0, dy = axis == 1, dz = axis == 2;
   const float2 a = load_voxel(v, gx, gy, gz), b = load_voxel(v, gx + dx, gy + dy, gz + dz);
   const double f0 = fabs((double)a.x), f1 = fabs((double)b.x);
-  const double vl = v.voxel_length, half = vl * 0.5;
+  const double vl = v.voxel_length, half = __dmul_rn(vl, 0.5), sum = __dadd_rn(f0, f1);
   // global (lattice) voxel index = window origin + window-relative index
-  double p[3] = {half + vl * (double)(v.b0[0] * GSB_BRICK + gx), half + vl * (double)(v.b0[1] * GSB_BRICK + gy),
-                 half + vl * (double)(v.b0[2] * GSB_BRICK + gz)};
-  p[axis] += f0 * vl / (f0 + f1);
+  double p[3] = {__dadd_rn(half, __dmul_rn(vl, (double)(v.b0[0] * GSB_BRICK + gx))),
+                 __dadd_rn(half, __dmul_rn(vl, (double)(v.b0[1] * GSB_BRICK + gy))),
+                 __dadd_rn(half, __dmul_rn(vl, (double)(v.b0[2] * GSB_BRICK + gz)))};
+  p[axis] = __dadd_rn(p[axis], __ddiv_rn(__dmul_rn(f0, vl), sum));
   xyz[3 * i] = p[0];
   xyz[3 * i + 1] = p[1];
   xyz[3 * i + 2] = p[2];
@@ -142,47 +146,55 @@ __global__ void __launch_bounds__(256) mc_vertices_kernel(const VolView v, const
     const size_t ia = voxel_address(v, gx, gy, gz), ib = voxel_address(v, gx + dx, gy + dy, gz + dz);
     const float4 zero = make_float4(0.f, 0.f, 0.f, 0.f);
     const float4 c0 = ia == (size_t)-1 ? zero : v.color[ia], c1 = ib == (size_t)-1 ? zero : v.color[ib];
-    const double inv = 1.0 / (f0 + f1);
-    rgb[3 * i] = (float)((f1 * ((double)c0.x / 255.0) + f0 * ((double)c1.x / 255.0)) * inv);
-    rgb[3 * i + 1] = (float)((f1 * ((double)c0.y / 255.0) + f0 * ((double)c1.y / 255.0)) * inv);
-    rgb[3 * i + 2] = (float)((f1 * ((double)c0.z / 255.0) + f0 * ((double)c1.z / 255.0)) * inv);
-  }
-}
-
-// Area-weighted vertex normals (TriangleMesh::ComputeVertexNormals: unnormalised triangle
-// normals are summed per vertex, then normalised).
-__global__ void __launch_bounds__(256) mesh_accumulate_normals_kernel(const double* __restrict__ xyz,
-                                                                      const long long* __restrict__ tris, long long nt,
-                                                                      double* __restrict__ normals) {
-  const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (t >= nt) return;
-  const long long i0 = tris[3 * t], i1 = tris[3 * t + 1], i2 = tris[3 * t + 2];
-  const double ax = xyz[3 * i1] - xyz[3 * i0], ay = xyz[3 * i1 + 1] - xyz[3 * i0 + 1], az = xyz[3 * i1 + 2] - xyz[3 * i0 + 2];
-  const double bx = xyz[3 * i2] - xyz[3 * i0], by = xyz[3 * i2 + 1] - xyz[3 * i0 + 1], bz = xyz[3 * i2 + 2] - xyz[3 * i0 + 2];
-  const double nx = ay * bz - az * by, ny = az * bx - ax * bz, nz = ax * by - ay * bx;
-  const long long ids[3] = {i0, i1, i2};
+    const float k0[3] = {c0.x, c0.y, c0.z}, k1[3] = {c1.x, c1.y, c1.z};
 #pragma unroll
-  for (int k = 0; k < 3; ++k) {
-    atomicAdd(&normals[3 * ids[k]], nx);
-    atomicAdd(&normals[3 * ids[k] + 1], ny);
-    atomicAdd(&normals[3 * ids[k] + 2], nz);
+    for (int k = 0; k < 3; ++k) {
+      const double w0 = __dmul_rn(f1, __ddiv_rn((double)k0[k], 255.0)), w1 = __dmul_rn(f0, __ddiv_rn((double)k1[k], 255.0));
+      rgb[3 * i + k] = __ddiv_rn(__dadd_rn(w0, w1), sum);
+    }
   }
 }
 
-__global__ void __launch_bounds__(256) mesh_normalize_kernel(double* __restrict__ normals, long long nv) {
+// Vertex normals of TriangleMesh::ComputeVertexNormals(normalized=true), bit for bit and run to run.  Open3D sums the
+// unnormalised triangle normals (v1-v0).cross(v2-v0) into each vertex of triangle 0, 1, 2, ... in turn, then calls
+// MeshBase::NormalizeNormals().  One thread per vertex walks its incidences (positions 3*t+k of the flattened triangle
+// array, in ascending order) and adds them in that same order, one rounding per operation -- no atomics, so the sum
+// does not depend on scheduling.  NormalizeNormals() is Eigen's normalize(), which (Eigen >= 3.3, MatrixBase::normalize
+// in Dot.h) divides by sqrt(squaredNorm()) only if squaredNorm() > 0, followed by Open3D's `isnan(n(0))` -> (0,0,1);
+// a zero sum therefore stays (0,0,0).  squaredNorm() of a Vector3d is Eigen's vectorised redux: (x*x + y*y) + z*z.
+__global__ void __launch_bounds__(256) mesh_vertex_normals_kernel(const double* __restrict__ xyz,
+                                                                  const long long* __restrict__ tris,
+                                                                  const long long* __restrict__ incidence,
+                                                                  const long long* __restrict__ offsets, long long nv,
+                                                                  double* __restrict__ normals) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= nv) return;
-  const double x = normals[3 * i], y = normals[3 * i + 1], z = normals[3 * i + 2];
-  const double len = sqrt(x * x + y * y + z * z);
-  if (len > 0.0) {
-    normals[3 * i] = x / len;
-    normals[3 * i + 1] = y / len;
-    normals[3 * i + 2] = z / len;
-  } else {  // Open3D leaves (0,0,1) for degenerate normals
-    normals[3 * i] = 0.0;
-    normals[3 * i + 1] = 0.0;
-    normals[3 * i + 2] = 1.0;
+  double sx = 0.0, sy = 0.0, sz = 0.0;
+  for (long long j = offsets[i], end = offsets[i + 1]; j < end; ++j) {
+    const long long t = incidence[j] / 3;
+    const long long i0 = tris[3 * t], i1 = tris[3 * t + 1], i2 = tris[3 * t + 2];
+    const double x0 = xyz[3 * i0], y0 = xyz[3 * i0 + 1], z0 = xyz[3 * i0 + 2];
+    const double ax = __dsub_rn(xyz[3 * i1], x0), ay = __dsub_rn(xyz[3 * i1 + 1], y0), az = __dsub_rn(xyz[3 * i1 + 2], z0);
+    const double bx = __dsub_rn(xyz[3 * i2], x0), by = __dsub_rn(xyz[3 * i2 + 1], y0), bz = __dsub_rn(xyz[3 * i2 + 2], z0);
+    sx = __dadd_rn(sx, __dsub_rn(__dmul_rn(ay, bz), __dmul_rn(az, by)));
+    sy = __dadd_rn(sy, __dsub_rn(__dmul_rn(az, bx), __dmul_rn(ax, bz)));
+    sz = __dadd_rn(sz, __dsub_rn(__dmul_rn(ax, by), __dmul_rn(ay, bx)));
   }
+  const double sq = __dadd_rn(__dadd_rn(__dmul_rn(sx, sx), __dmul_rn(sy, sy)), __dmul_rn(sz, sz));
+  if (sq > 0.0) {
+    const double len = __dsqrt_rn(sq);
+    sx = __ddiv_rn(sx, len);
+    sy = __ddiv_rn(sy, len);
+    sz = __ddiv_rn(sz, len);
+  }
+  if (isnan(sx)) {
+    sx = 0.0;
+    sy = 0.0;
+    sz = 1.0;
+  }
+  normals[3 * i] = sx;
+  normals[3 * i + 1] = sy;
+  normals[3 * i + 2] = sz;
 }
 
 VolView view_of(const GsbVolume* vol, const int32_t* window) {
@@ -202,13 +214,21 @@ VolView view_of(const GsbVolume* vol, const int32_t* window) {
   return v;
 }
 
-bool window_ok(const int32_t* w) {
-  if (!w) return false;
+// GSB_OK, or the error for a key window that is malformed or too large.  A window may span the whole lattice plus the
+// +1 brick past its end: 2^21 + 1 bricks per axis.
+int window_check(const char* who, const int32_t* w) {
+  if (!w) return fail(GSB_ERR_INVALID, "%s: bad arguments", who);
   for (int k = 0; k < 3; ++k)
-    if (w[3 + k] <= 0 || w[3 + k] > (1 << 21)) return false;
+    if (w[3 + k] <= 0 || w[3 + k] > (1 << 21) + 1 || w[k] < -kBrickBias || w[k] >= kBrickBias)
+      return fail(GSB_ERR_INVALID, "%s: bad key window", who);
   // keys = ((gx*NY + gy)*NZ + gz)*3 + axis must fit 63 bits
   const double vox = 16.0 * 16.0 * 16.0 * (double)w[3] * (double)w[4] * (double)w[5] * 3.0;
-  return vox < 9.0e18;
+  if (vox >= 9.0e18)
+    return fail(GSB_ERR_INVALID,
+                "%s: the bounding box of the open bricks (%d x %d x %d bricks) is too large for 63-bit edge keys "
+                "(16^3 * nbx * nby * nbz * 3 must be < 9e18)",
+                who, w[3], w[4], w[5]);
+  return GSB_OK;
 }
 
 }  // namespace
@@ -221,7 +241,8 @@ extern "C" {
 int gsb_mesh_count(const GsbVolume* vol, const int32_t* window, const uint32_t* bricks, uint32_t n_bricks, uint32_t* tri_counts,
                    void* stream_v) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
-  if (!vol || !window_ok(window) || (n_bricks && (!bricks || !tri_counts))) return fail(GSB_ERR_INVALID, "mesh_count: bad arguments");
+  if (!vol || (n_bricks && (!bricks || !tri_counts))) return fail(GSB_ERR_INVALID, "mesh_count: bad arguments");
+  if (const int rc = window_check("mesh_count", window)) return rc;
   if (n_bricks == 0) return GSB_OK;
   mc_brick_kernel<<<n_bricks, 256, 0, stream>>>(view_of(vol, window), bricks, 0, tri_counts, nullptr, nullptr);
   count_launch();
@@ -231,8 +252,8 @@ int gsb_mesh_count(const GsbVolume* vol, const int32_t* window, const uint32_t* 
 int gsb_mesh_emit(const GsbVolume* vol, const int32_t* window, const uint32_t* bricks, uint32_t n_bricks, const int64_t* tri_offsets,
                   int64_t* edge_keys, void* stream_v) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
-  if (!vol || !window_ok(window) || (n_bricks && (!bricks || !tri_offsets || !edge_keys)))
-    return fail(GSB_ERR_INVALID, "mesh_emit: bad arguments");
+  if (!vol || (n_bricks && (!bricks || !tri_offsets || !edge_keys))) return fail(GSB_ERR_INVALID, "mesh_emit: bad arguments");
+  if (const int rc = window_check("mesh_emit", window)) return rc;
   if (n_bricks == 0) return GSB_OK;
   mc_brick_kernel<<<n_bricks, 256, 0, stream>>>(view_of(vol, window), bricks, 1, nullptr, reinterpret_cast<const long long*>(tri_offsets),
                                                 reinterpret_cast<long long*>(edge_keys));
@@ -240,10 +261,11 @@ int gsb_mesh_emit(const GsbVolume* vol, const int32_t* window, const uint32_t* b
   return check_launch("mc_brick_kernel(emit)", stream, false);
 }
 
-int gsb_mesh_vertices(const GsbVolume* vol, const int32_t* window, const int64_t* keys, int64_t n, double* xyz, float* rgb,
+int gsb_mesh_vertices(const GsbVolume* vol, const int32_t* window, const int64_t* keys, int64_t n, double* xyz, double* rgb,
                       void* stream_v) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
-  if (!vol || !window_ok(window) || n < 0 || (n && (!keys || !xyz))) return fail(GSB_ERR_INVALID, "mesh_vertices: bad arguments");
+  if (!vol || n < 0 || (n && (!keys || !xyz))) return fail(GSB_ERR_INVALID, "mesh_vertices: bad arguments");
+  if (const int rc = window_check("mesh_vertices", window)) return rc;
   if (n == 0) return GSB_OK;
   mc_vertices_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(view_of(vol, window), reinterpret_cast<const long long*>(keys),
                                                                      n, xyz, rgb);
@@ -251,21 +273,18 @@ int gsb_mesh_vertices(const GsbVolume* vol, const int32_t* window, const int64_t
   return check_launch("mc_vertices_kernel", stream, false);
 }
 
-int gsb_mesh_vertex_normals(const double* xyz, int64_t n_vertices, const int64_t* triangles, int64_t n_triangles, double* normals,
-                            void* stream_v) {
+int gsb_mesh_vertex_normals(const double* xyz, int64_t n_vertices, const int64_t* triangles, int64_t n_triangles,
+                            const int64_t* incidence, const int64_t* incidence_offsets, double* normals, void* stream_v) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
-  if (n_vertices < 0 || n_triangles < 0 || (n_vertices && (!xyz || !normals)) || (n_triangles && !triangles))
+  if (n_vertices < 0 || n_triangles < 0 || (n_vertices && (!xyz || !normals || !incidence_offsets)) ||
+      (n_triangles && (!triangles || !incidence)))
     return fail(GSB_ERR_INVALID, "mesh_vertex_normals: bad arguments");
   if (n_vertices == 0) return GSB_OK;
-  GSB_CUDA_OK(cudaMemsetAsync(normals, 0, sizeof(double) * 3 * (size_t)n_vertices, stream));
-  if (n_triangles) {
-    mesh_accumulate_normals_kernel<<<(unsigned)((n_triangles + 255) / 256), 256, 0, stream>>>(
-        xyz, reinterpret_cast<const long long*>(triangles), n_triangles, normals);
-    count_launch();
-  }
-  mesh_normalize_kernel<<<(unsigned)((n_vertices + 255) / 256), 256, 0, stream>>>(normals, n_vertices);
+  mesh_vertex_normals_kernel<<<(unsigned)((n_vertices + 255) / 256), 256, 0, stream>>>(
+      xyz, reinterpret_cast<const long long*>(triangles), reinterpret_cast<const long long*>(incidence),
+      reinterpret_cast<const long long*>(incidence_offsets), n_vertices, normals);
   count_launch();
-  return check_launch("mesh normals", stream, false);
+  return check_launch("mesh_vertex_normals_kernel", stream, false);
 }
 
 }  // extern "C"

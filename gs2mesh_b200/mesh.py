@@ -19,6 +19,17 @@ from . import _lib
 from ._lib import ptr
 
 
+def color_to_uint8(colors):
+    """Open3D's utility::ColorToUint8, which its PLY writer applies to vertex colours:
+    uint8_t(std::round(std::min(1., std::max(0., c)) * 255.)).  std::round rounds halves away from zero (np.rint would
+    round them to even), and std::max(0., NaN) is 0."""
+    c = np.asarray(colors, dtype=np.float64)
+    c = np.where(c > 0.0, c, 0.0)
+    s = np.where(c < 1.0, c, 1.0) * 255.0
+    lo = np.floor(s)
+    return (lo + (s - lo >= 0.5)).astype(np.uint8)
+
+
 class TriangleMesh:
     """Minimal stand-in for open3d.geometry.TriangleMesh (the members tsdf_utils.py touches)."""
 
@@ -34,19 +45,28 @@ class TriangleMesh:
         self.vertices = (self.vertices - c) * float(scale) + c
         return self
 
-    # -- tsdf_utils.py:110 (area-weighted, normalised; TriangleMesh::ComputeVertexNormals)
+    # -- tsdf_utils.py:110 (area-weighted, normalised; TriangleMesh::ComputeVertexNormals, bit for bit)
     def compute_vertex_normals(self, device=None):
         nv, nt = len(self.vertices), len(self.triangles)
         if nv == 0:
             self.vertex_normals = np.zeros((0, 3))
             return self
+        if nt and (self.triangles.min() < 0 or self.triangles.max() >= nv):
+            raise ValueError("compute_vertex_normals: triangle vertex index out of range")
         dev = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
         with torch.cuda.device(dev):
             xyz = torch.as_tensor(self.vertices).to(dev).contiguous()
             tri = torch.as_tensor(self.triangles).to(dev).contiguous()
+            # vertex -> triangle incidence as CSR; the stable sort keeps each vertex's triangles in triangle order, the
+            # order Open3D adds them in
+            flat = tri.reshape(-1)
+            incidence = torch.sort(flat, stable=True).indices
+            offsets = torch.zeros(nv + 1, dtype=torch.int64, device=dev)
+            offsets[1:] = torch.cumsum(torch.bincount(flat, minlength=nv), 0)
             out = torch.empty(nv, 3, dtype=torch.float64, device=dev)
             stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-            _lib.check(_lib.lib().gsb_mesh_vertex_normals(ptr(xyz), nv, ptr(tri), nt, ptr(out), stream))
+            _lib.check(_lib.lib().gsb_mesh_vertex_normals(ptr(xyz), nv, ptr(tri), nt, ptr(incidence), ptr(offsets), ptr(out),
+                                                          stream))
             self.vertex_normals = out.cpu().numpy()
         return self
 
@@ -103,8 +123,7 @@ class TriangleMesh:
         if self.vertex_normals is not None and nv:
             vert["nx"], vert["ny"], vert["nz"] = self.vertex_normals.T
         if self.vertex_colors is not None and nv:
-            rgb = np.clip(np.rint(self.vertex_colors * 255.0), 0, 255).astype(np.uint8)
-            vert["red"], vert["green"], vert["blue"] = rgb.T
+            vert["red"], vert["green"], vert["blue"] = color_to_uint8(self.vertex_colors).T
         face = np.zeros(nt, dtype=[("n", "u1"), ("v", "<u4", (3,))])
         face["n"] = 3
         face["v"] = self.triangles.astype(np.uint32)
@@ -142,10 +161,10 @@ def extract_triangle_mesh(volume, with_colors: Optional[bool] = None) -> Triangl
         uniq, inverse = torch.unique(keys, return_inverse=True)  # vertex ids = rank of the edge key
         nv = int(uniq.numel())
         xyz = torch.empty(nv, 3, dtype=torch.float64, device=dev)
-        rgb = torch.empty(nv, 3, dtype=torch.float32, device=dev) if with_colors else None
+        rgb = torch.empty(nv, 3, dtype=torch.float64, device=dev) if with_colors else None
         _lib.check(L.gsb_mesh_vertices(volume._h, window, ptr(uniq.contiguous()), nv, ptr(xyz), ptr(rgb), stream))
         tris = inverse.reshape(-1, 3)
-        mesh = TriangleMesh(xyz.cpu().numpy(), tris.cpu().numpy(), None if rgb is None else rgb.double().cpu().numpy())
+        mesh = TriangleMesh(xyz.cpu().numpy(), tris.cpu().numpy(), None if rgb is None else rgb.cpu().numpy())
         mesh.edge_keys = uniq.cpu().numpy()  # (voxel index inside `key_window` * 3 + axis) per vertex, for tests
         mesh.key_window = (tuple(int(v) for v in lo), tuple(int(v) for v in (hi - lo + 2)))  # (brick origin, brick count)
     return mesh

@@ -304,19 +304,23 @@ void gsb_comm_destroy(void* nccl_comm);
  * key = ((gx*NY + gy)*NZ + gz)*3 + axis over the voxel grid of `window` (host int32[6]: brick origin, brick count of a
  * box containing every listed brick and its +1 neighbours, e.g. the bounding box of the pool + 1); the caller
  * sorts/uniques the keys (that is the de-duplication Open3D does with a hash map) and asks for the attributes of the
- * unique edges.
+ * unique edges.  The keys must fit 63 bits: 16^3 * nbx * nby * nbz * 3 < 9e18, otherwise GSB_ERR_INVALID.
  *   gsb_mesh_count    tri_counts[b]  = triangles produced by brick b
  *   gsb_mesh_emit     edge_keys[3*t..3*t+2] for every triangle, brick b writing from tri_offsets[b]
- *   gsb_mesh_vertices xyz (fp64, Open3D's interpolation) and rgb in [0,1] (or NULL) of n unique keys
- *   gsb_mesh_vertex_normals area-weighted vertex normals (fp64 [n_vertices,3]) of an indexed mesh */
+ *   gsb_mesh_vertices xyz and rgb in [0,1] (or NULL) of n unique keys, fp64 [n,3] each, equal to Open3D's doubles
+ *                     (one rounding per operation in Open3D's order)
+ *   gsb_mesh_vertex_normals TriangleMesh::ComputeVertexNormals() (fp64 [n_vertices,3]) of an indexed mesh, deterministic.
+ *                     The caller passes the vertex -> triangle incidence as CSR: incidence = the positions 3*t+k of
+ *                     triangles[] sorted by vertex id, ties in ascending position (a stable sort of the flattened
+ *                     array), incidence_offsets[n_vertices + 1] = where each vertex's run starts. */
 int gsb_mesh_count(const GsbVolume* vol, const int32_t* window, const uint32_t* bricks, uint32_t n_bricks, uint32_t* tri_counts,
                    void* stream);
 int gsb_mesh_emit(const GsbVolume* vol, const int32_t* window, const uint32_t* bricks, uint32_t n_bricks, const int64_t* tri_offsets,
                   int64_t* edge_keys, void* stream);
-int gsb_mesh_vertices(const GsbVolume* vol, const int32_t* window, const int64_t* keys, int64_t n, double* xyz, float* rgb,
+int gsb_mesh_vertices(const GsbVolume* vol, const int32_t* window, const int64_t* keys, int64_t n, double* xyz, double* rgb,
                       void* stream);
-int gsb_mesh_vertex_normals(const double* xyz, int64_t n_vertices, const int64_t* triangles, int64_t n_triangles, double* normals,
-                            void* stream);
+int gsb_mesh_vertex_normals(const double* xyz, int64_t n_vertices, const int64_t* triangles, int64_t n_triangles,
+                            const int64_t* incidence, const int64_t* incidence_offsets, double* normals, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Mesh-quality evaluation (evaluation/DTU/eval_code/eval.py, MobileBrick evaluate.py) without Open3D / sklearn.
