@@ -26,9 +26,22 @@
 namespace gsb {
 namespace {
 
-// counters (uint32[8]): [0] entries queued this frame  [1] bricks dropped this frame (pool full / index out of range)
+// counters (uint32[8]): [0] entries queued this frame  [1] bricks dropped this frame (pool full)
+//                       [2] brick-box cells outside the lattice this frame
 //                       [4] pool slots in use (persistent)  [5] bricks dropped since creation (persistent)
-constexpr int kCntQueued = 0, kCntDropped = 1, kCntPool = 4, kCntDroppedTotal = 5;
+//                       [6] brick-box cells outside the lattice since creation (persistent)
+// Every drop and every out-of-range cell is added to its per-frame word and its persistent word with atomics where it is
+// found, so no kernel folds one into the other.
+constexpr int kCntQueued = 0, kCntDropped = 1, kCntOutOfRange = 2, kCntPool = 4, kCntDroppedTotal = 5, kCntOutOfRangeTotal = 6;
+
+__device__ __forceinline__ void count_dropped(uint32_t* counters) {
+  atomicAdd(&counters[kCntDropped], 1u);
+  atomicAdd(&counters[kCntDroppedTotal], 1u);
+}
+__device__ __forceinline__ void count_out_of_range(uint32_t* counters) {
+  atomicAdd(&counters[kCntOutOfRange], 1u);
+  atomicAdd(&counters[kCntOutOfRangeTotal], 1u);
+}
 
 struct HashView {
   unsigned long long* keys;
@@ -40,7 +53,9 @@ struct HashView {
 
 // position of brick (bx,by,bz) in the table, inserting it (and giving it the next pool slot) if absent; kSlotNone if the
 // brick cannot be stored.  The pool slot of a fresh key is written by the inserting thread with a plain store: readers of
-// hash_vals are always a later kernel.
+// hash_vals are always a later kernel.  Threads that pass the pool check together can all insert; those whose slot lands
+// past the pool leave a dead key (hash_vals = kSlotNone) and still return its position.  A dead key is therefore counted
+// as dropped by whoever reads its slot: integrate_kernel, count_dead_kernel (touch) and resolve_slots_kernel.
 __device__ __forceinline__ uint32_t brick_find_or_insert(const HashView& hv, uint32_t* __restrict__ counters, int bx, int by,
                                                          int bz) {
   if (!brick_key_ok(bx, by, bz)) return kSlotNone;
@@ -148,7 +163,7 @@ __global__ void __launch_bounds__(256) mark_bricks_kernel(const MarkParams m, co
         if (brick_key_ok(bx[u], by[u], bz[u])) {
           key[u] = brick_key(bx[u], by[u], bz[u]);
         } else {
-          atomicAdd(&counters[kCntDropped], 1u);
+          count_out_of_range(counters);  // not a pool drop: a larger pool cannot hold it
           mine = false;
         }
       }
@@ -167,7 +182,7 @@ __global__ void __launch_bounds__(256) mark_bricks_kernel(const MarkParams m, co
       if (seen[u] != key[u]) {  // not at its home slot (collision or not yet opened): walk / insert
         hh = brick_find_or_insert(hv, counters, bx[u], by[u], bz[u]);
         if (hh == kSlotNone) {
-          atomicAdd(&counters[kCntDropped], 1u);  // reported by gsb_tsdf_last_stats; the stage class grows the pool
+          count_dropped(counters);  // reported by gsb_tsdf_last_stats; the stage class grows the pool
           continue;
         }
         st[u] = hv.stamp[hh];
@@ -204,7 +219,9 @@ __device__ __forceinline__ void st_stream(float4* p, const float4& v) {
 
 // UniformTSDFVolume::IntegrateWithDepthToCameraDistanceMultiplier, one voxel, split in two so that
 // the depth-image gathers of all of a thread's voxels can be in flight together:
-//   project_voxel: camera-space point -> packed pixel (v << 16 | u), or -1 if the voxel is skipped
+//   project_voxel: camera-space point -> packed pixel (v << 16 | u), or -1 if the voxel is skipped.  The packing holds
+//                  u < 65536 and v < 32768 (GSB_TSDF_MAX_WIDTH / _HEIGHT, checked by the entry points), and then
+//                  v * W + u < 2^31 as well.
 //   fuse_voxel:    depth sample -> truncated distance -> running weighted mean
 __device__ __forceinline__ int project_voxel(const FrameParams& f, float pcx, float pcy, float pcz) {
   if (pcz <= 0.f) return -1;
@@ -264,8 +281,6 @@ __global__ void __launch_bounds__(kIntThreads, kMinBlocks) integrate_kernel(cons
                                                                   const uint32_t* __restrict__ hash_vals, uint32_t pool) {
   // a frame cannot queue more entries than the list holds (one per pool slot + the few a full pool refused)
   const uint32_t n = counters[kCntQueued];
-  if (blockIdx.x == 0 && threadIdx.x == 0 && counters[kCntDropped] != 0)
-    counters[kCntDroppedTotal] += counters[kCntDropped];  // the frame's drop count is final: mark_bricks ran before
   const int t = threadIdx.x;
   // thread -> voxel pair: pair q = pass*256 + t, first voxel 2q = (x, y, z) with
   //   x = 2*pass + (t >> 7), y = (t >> 3) & 15, z = 2 * (t & 7)
@@ -274,7 +289,10 @@ __global__ void __launch_bounds__(kIntThreads, kMinBlocks) integrate_kernel(cons
   for (uint32_t it = blockIdx.x; it < n; it += gridDim.x) {
     const uint32_t entry = list[it];
     const uint32_t brick = hash_vals[entry];  // pool slot
-    if (brick >= pool) continue;              // the pool was full when this brick was opened (counted as dropped)
+    if (brick >= pool) {                      // dead key: the pool was full when this brick was opened
+      if (t == 0) count_dropped(counters);   // each entry is listed once per frame, so counted once per frame
+      continue;
+    }
     int bx, by, bz;
     brick_unkey(hash_keys[entry], bx, by, bz);
     const double ox = (double)bx * f.unit_length;  // origin = index * unit_length (OpenVolumeUnit)
@@ -495,23 +513,36 @@ __global__ void __launch_bounds__(256) find_bricks_kernel(const HashView hv, uin
   if (i >= n || (n_dev != nullptr && i >= *n_dev)) return;
   const int bx = indices[4 * (size_t)i], by = indices[4 * (size_t)i + 1], bz = indices[4 * (size_t)i + 2];
   uint32_t h = kSlotNone;
-  if (insert) {
+  if (insert && !brick_key_ok(bx, by, bz)) {
+    count_out_of_range(counters);
+  } else if (insert) {
     h = brick_find_or_insert(hv, counters, bx, by, bz);
-    if (h == kSlotNone) atomicAdd(&counters[kCntDropped], 1u);
+    if (h == kSlotNone) count_dropped(counters);  // a dead key (h != kSlotNone) is counted by resolve_slots_kernel
   } else if (brick_key_ok(bx, by, bz)) {
     h = brick_find(hv.keys, hv.mask, brick_key(bx, by, bz));
   }
   if (entries) entries[i] = h;
   if (slots) slots[i] = kSlotNone;  // resolved by resolve_slots_kernel once every insertion of this launch has landed
 }
+// insert != 0: an entry without a pool slot (a dead key, found or just left by brick_find_or_insert) is a dropped brick
 __global__ void __launch_bounds__(256) resolve_slots_kernel(const uint32_t* __restrict__ vals, const uint32_t* __restrict__ entries,
                                                             uint32_t n, const uint32_t* __restrict__ n_dev, uint32_t pool,
+                                                            int insert, uint32_t* __restrict__ counters,
                                                             uint32_t* __restrict__ slots) {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n || (n_dev != nullptr && i >= *n_dev)) return;
   const uint32_t h = entries[i];
   const uint32_t s = h == kSlotNone ? kSlotNone : vals[h];
+  if (insert && h != kSlotNone && s >= pool) count_dropped(counters);
   slots[i] = s < pool ? s : kSlotNone;
+}
+
+// gsb_tsdf_touch: the dead keys among the frame's listed entries (integrate_kernel counts them itself when it runs)
+__global__ void __launch_bounds__(256) count_dead_kernel(const uint32_t* __restrict__ list, const uint32_t* __restrict__ vals,
+                                                         uint32_t pool, uint32_t* __restrict__ counters) {
+  const uint32_t n = counters[kCntQueued];
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x)
+    if (vals[list[i]] >= pool) count_dropped(counters);
 }
 
 __global__ void copy_stats_kernel(uint32_t* counters, uint32_t frame, uint32_t* out) {
@@ -520,7 +551,9 @@ __global__ void copy_stats_kernel(uint32_t* counters, uint32_t frame, uint32_t* 
   out[2] = frame;
   out[3] = counters[kCntPool];
   out[4] = counters[kCntDroppedTotal];
-  out[5] = out[6] = out[7] = 0;
+  out[5] = counters[kCntOutOfRange];
+  out[6] = counters[kCntOutOfRangeTotal];
+  out[7] = 0;
 }
 
 // general 4x4 inverse in double (Gauss-Jordan with partial pivoting)
@@ -672,26 +705,32 @@ static int run_mark(GsbVolume* vol, const float* depth, int32_t width, int32_t h
   return check_launch("mark_bricks_kernel", stream, false);
 }
 
-__global__ void fold_drops_kernel(uint32_t* counters) {
-  if (counters[kCntDropped] != 0) counters[kCntDroppedTotal] += counters[kCntDropped];
+// the packed pixel index of integrate_kernel (project_voxel) holds u < 65536, v < 32768
+static int check_frame_size(const char* fn, int32_t width, int32_t height) {
+  if (width > GSB_TSDF_MAX_WIDTH || height > GSB_TSDF_MAX_HEIGHT)
+    return fail(GSB_ERR_INVALID, "%s: frame %dx%d exceeds the supported %dx%d (width x height)", fn, width, height,
+                GSB_TSDF_MAX_WIDTH, GSB_TSDF_MAX_HEIGHT);
+  return GSB_OK;
 }
 
 int gsb_tsdf_touch(GsbVolume* vol, const float* depth, int32_t width, int32_t height, double fx, double fy, double cx, double cy,
                    const double* extrinsic, void* stream_v) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
   if (!vol || !depth || !extrinsic || width <= 0 || height <= 0) return fail(GSB_ERR_INVALID, "tsdf_touch: bad arguments");
-  double unit_length = 0;
   int rc;
+  if ((rc = check_frame_size("tsdf_touch", width, height))) return rc;
+  double unit_length = 0;
   if ((rc = run_mark(vol, depth, width, height, fx, fy, cx, cy, extrinsic, stream, &unit_length))) return rc;
-  fold_drops_kernel<<<1, 1, 0, stream>>>(vol->d.counters);
+  count_dead_kernel<<<num_sms(), 256, 0, stream>>>(vol->d.brick_list, vol->d.hash_vals, vol->d.pool_bricks, vol->d.counters);
   count_launch();
-  return check_launch("fold_drops_kernel", stream, false);
+  return check_launch("count_dead_kernel", stream, false);
 }
 
 int gsb_tsdf_integrate(GsbVolume* vol, const float* depth, const uint8_t* rgb, int32_t width, int32_t height, double fx,
                        double fy, double cx, double cy, const double* extrinsic, void* stream_v) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
   if (!vol || !depth || !extrinsic || width <= 0 || height <= 0) return fail(GSB_ERR_INVALID, "tsdf_integrate: bad arguments");
+  if (int rc = check_frame_size("tsdf_integrate", width, height)) return rc;
   const GsbVolumeDesc& d = vol->d;
   double unit_length = 0;
   int rc;
@@ -780,7 +819,8 @@ int gsb_tsdf_find_bricks(GsbVolume* vol, const int32_t* indices, uint32_t n, int
   if (n == 0) return GSB_OK;
   const GsbVolumeDesc& d = vol->d;
   find_bricks_kernel<<<(n + 255) / 256, 256, 0, stream>>>(hash_view(d), d.counters, indices, n, nullptr, insert, slots, scratch);
-  resolve_slots_kernel<<<(n + 255) / 256, 256, 0, stream>>>(d.hash_vals, scratch, n, nullptr, d.pool_bricks, slots);
+  resolve_slots_kernel<<<(n + 255) / 256, 256, 0, stream>>>(d.hash_vals, scratch, n, nullptr, d.pool_bricks, insert, d.counters,
+                                                            slots);
   count_launch(2);
   return check_launch("find_bricks_kernel", stream, false);
 }

@@ -35,6 +35,7 @@ def default_window(resolution: int = 512):
 
 
 DEFAULT_POOL_BRICKS = 1 << 15  # 32768 bricks = 1 GiB of (tsdf, weight) + 2 GiB of colour; grown on demand
+LATTICE_LIMIT = 1 << 20  # brick lattice indices lie in [-2^20, 2^20) per axis (21-bit hash keys)
 
 
 class TSDFVolume:
@@ -195,13 +196,16 @@ class TSDFVolume:
         self.integrate(depth, rgb, width, height, fx, fy, cx, cy, extrinsic_w2c)
 
     def pool_stats(self):
-        """dict(touched, dropped, frame, bricks, dropped_total) -- synchronises.  `dropped` counts bricks the last integrate
-        could not open (pool exhausted); `dropped_total` since creation / reset."""
+        """dict(touched, dropped, frame, bricks, dropped_total, out_of_range, out_of_range_total) -- synchronises.
+        `dropped` counts bricks the last integrate could not store for want of pool slots; `dropped_total` since creation /
+        reset.  `out_of_range` counts the brick-box cells of the last integrate whose lattice index lies outside
+        [-2^20, 2^20) (one per sampled pixel and cell); no pool can hold those."""
         out = torch.zeros(8, dtype=torch.int32, device=self.device)
         with torch.cuda.device(self.device):
             _lib.check(self._L.gsb_tsdf_last_stats(self._h, ptr(out), self._stream()))
         v = out.cpu().numpy().astype(np.int64) & 0xFFFFFFFF
-        return dict(touched=int(v[0]), dropped=int(v[1]), frame=int(v[2]), bricks=int(v[3]), dropped_total=int(v[4]))
+        return dict(touched=int(v[0]), dropped=int(v[1]), frame=int(v[2]), bricks=int(v[3]), dropped_total=int(v[4]),
+                    out_of_range=int(v[5]), out_of_range_total=int(v[6]))
 
     def last_stats(self):
         """(bricks touched, bricks dropped, frame id) of the last integrate (syncs)."""
@@ -214,8 +218,14 @@ class TSDFVolume:
 
     def ensure_capacity(self):
         """After a batch of integrations: True if every brick found room.  Otherwise the pool is doubled (content kept, the
-        dropped-bricks counter cleared) and False is returned -- the views since the last check must be integrated again."""
+        dropped-bricks counter cleared) and False is returned -- the views since the last check must be integrated again.
+        Raises RuntimeError, without growing, if some brick lay outside the lattice range: integrating again cannot help."""
         s = self.pool_stats()
+        if s["out_of_range_total"]:
+            lim = LATTICE_LIMIT * BRICK * self.voxel_length
+            raise RuntimeError(f"TSDFVolume: {s['out_of_range_total']} brick-box cells lie outside the brick lattice range "
+                               f"[-2^20, 2^20) per axis (|coordinate| >= {lim:.6g} at voxel_length {self.voxel_length:.6g}); "
+                               "such bricks cannot be stored")
         if s["dropped_total"] == 0:
             return True
         self.grow()

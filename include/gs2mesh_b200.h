@@ -191,8 +191,10 @@ int gsb_image_to_u8(const float* chw, int32_t width, int32_t height, uint8_t* hw
  * All arrays are caller-allocated device memory (the library never allocates):
  *   tsdf_weight / color / brick_index / hash_vals / hash_stamp / brick_list / counters zero-initialised,
  *   hash_keys initialised to all-ones bytes (0xFF).
- * Lattice indices must lie in [-2^20, 2^20) per axis.  When the pool is exhausted further bricks are dropped and counted
- * (gsb_tsdf_last_stats); the caller grows the pool and integrates again. */
+ * Lattice indices must lie in [-2^20, 2^20) per axis: cells of a brick box outside that range are never stored and are
+ * counted apart from pool drops (counters[2] / [6]), since a larger pool cannot hold them.  When the pool is exhausted
+ * further bricks are dropped and counted (counters[1] / [5], gsb_tsdf_last_stats); the caller grows the pool and
+ * integrates again. */
 typedef struct GsbVolumeDesc {
   double voxel_length;
   double sdf_trunc;
@@ -206,7 +208,9 @@ typedef struct GsbVolumeDesc {
   uint32_t* hash_stamp;    /* device [hash_slots]      last frame id that queued the entry             */
   uint32_t* brick_list;    /* device [hash_slots]      scratch: entries touched by the current frame   */
   uint32_t* counters;      /* device [8]  [0] entries queued this frame, [1] bricks dropped this frame,
-                                          [4] pool slots in use, [5] bricks dropped since creation     */
+                                          [2] brick-box cells outside the lattice this frame,
+                                          [4] pool slots in use, [5] bricks dropped since creation,
+                                          [6] brick-box cells outside the lattice since creation       */
 } GsbVolumeDesc;
 
 typedef struct GsbVolume GsbVolume; /* opaque; owns no device memory */
@@ -231,9 +235,15 @@ int gsb_tsdf_prepare_depth(const float* depth_in, const float* final_T, const ui
 int gsb_mask_morphology(const uint8_t* mask_in, int32_t width, int32_t height, int32_t kernel_size, int32_t dilate,
                         uint8_t* mask_out, void* stream);
 
+/* Largest frame gsb_tsdf_integrate / gsb_tsdf_touch accept (larger ones fail with GSB_ERR_INVALID): the voxel update
+ * packs the pixel it samples as (v << 16) | u in one int. */
+#define GSB_TSDF_MAX_WIDTH 65536
+#define GSB_TSDF_MAX_HEIGHT 32768
+
 /* volume.integrate(rgbd, intrinsic, extrinsic): depth = prepared float depth [H,W] (device),
  * rgb = uint8 [H,W,3] (device) or NULL, extrinsic_w2c = row-major double[16] on the HOST
- * (what tsdf_utils.py:107 passes: inv(left_camera['extrinsic'])). */
+ * (what tsdf_utils.py:107 passes: inv(left_camera['extrinsic'])).  width <= GSB_TSDF_MAX_WIDTH,
+ * height <= GSB_TSDF_MAX_HEIGHT. */
 int gsb_tsdf_integrate(GsbVolume* vol, const float* depth, const uint8_t* rgb, int32_t width, int32_t height, double fx,
                        double fy, double cx, double cy, const double* extrinsic_w2c, void* stream);
 
@@ -260,8 +270,10 @@ int gsb_tsdf_export_dense(const GsbVolume* vol, const int32_t* brick_origin, con
                           float* weight, void* stream);
 
 /* Statistics, read back asynchronously into `out` (device or pinned host, uint32[8]): [0] bricks touched by the last
- * integrate, [1] bricks it had to drop (pool exhausted / index out of range), [2] frame id, [3] pool slots in use,
- * [4] bricks dropped since creation. */
+ * integrate, [1] bricks it had to drop (pool exhausted, including keys left without a slot by an earlier overflow),
+ * [2] frame id, [3] pool slots in use, [4] bricks dropped since creation, [5] brick-box cells of the last integrate outside
+ * the lattice range [-2^20, 2^20) (one per sampled pixel and cell, not de-duplicated), [6] the same since creation.
+ * gsb_tsdf_find_bricks with insert != 0 adds its drops and out-of-range indices to the same words. */
 int gsb_tsdf_last_stats(const GsbVolume* vol, uint32_t* out, void* stream);
 
 /* ------------------------------------------------------------------------------------------

@@ -171,7 +171,8 @@ def _tsdf_lib():
 
 def tsdf_set_variant(bits: int) -> None:
     """Sensitivity study of the restatement's two DOUBT points (oracle/tsdf_oracle.cpp): bit 0 pairwise 4x4*4x1 sum,
-    bit 1 `sdf / trunc`, bit 2 FMA-contracted product.  0 restores the restatement.  Process-wide: reset after use."""
+    bit 1 `sdf / trunc`, bit 2 FMA-contracted product; bit 3 keeps colour as the CUDA kernel's fp32 running mean instead
+    of Open3D's fp64.  0 restores the restatement.  Process-wide: reset after use."""
     _tsdf_lib().orc_tsdf_set_variant(int(bits))
 
 

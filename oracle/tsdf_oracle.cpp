@@ -77,6 +77,8 @@ inline int floor_div(double p, double len) { return (int)std::floor(p / len); }
 //          x86-64 build of Eigen 3.4 instantiates for aligned Matrix4f * Vector4f
 //   bit 1: sdf / trunc instead of sdf * (1 / trunc)
 //   bit 2: the product contracted to fused multiply-adds (a wheel built with -mfma)
+//   bit 3: colour kept as the fp32 running mean the CUDA kernel computes, (c*w + rgb) / (w + 1) with one rounding per
+//          operation, instead of Open3D's fp64 colour (tests pin the kernel's colour bit for bit with it)
 int g_variant = 0;
 
 // UniformTSDFVolume::IntegrateWithDepthToCameraDistanceMultiplier for one 16^3 unit.
@@ -123,8 +125,13 @@ void integrate_unit(Unit& u, const Volume& vol, const float* depth, const uint8_
           u.tsdf[ind] = (u.tsdf[ind] * w + t) / (w + 1.0f);
           if (vol.with_color && rgb) {
             const uint8_t* c = rgb + 3 * ((size_t)vi * W + ui);
-            for (int k = 0; k < 3; ++k)
-              u.color[3 * (size_t)ind + k] = (u.color[3 * (size_t)ind + k] * w + (double)c[k]) / (w + 1.0f);
+            for (int k = 0; k < 3; ++k) {
+              double& col = u.color[3 * (size_t)ind + k];
+              if (g_variant & 8)
+                col = (double)(((float)col * w + (float)c[k]) / (w + 1.0f));
+              else
+                col = (col * w + (double)c[k]) / (w + 1.0f);
+            }
           }
           u.weight[ind] = w + 1.0f;
         }
