@@ -112,6 +112,9 @@ SIGNATURES = {
     "gsb_eval_mask_dilate_disk": (C.c_int, [_vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _vp, _vp, _vp]),
     "gsb_eval_cull_vertices_by_masks": (C.c_int, [_vp, C.c_int64, _vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                                   _vp, _vp, _vp]),
+    "gsb_stereo_pack_inputs": (C.c_int, [_vp, _vp, C.c_int32, C.c_int32, _vp, _vp]),
+    "gsb_stereo_disparities": (C.c_int, [_vp, _vp, C.c_int32, C.c_int32, C.c_float, _vp, _vp, _vp]),
+    "gsb_stereo_occlusion_depth": (C.c_int, [_vp, _vp, C.c_int32, C.c_int32, C.c_int64, C.c_double, C.c_float, _vp, _vp, _vp]),
 }
 
 _lib = None

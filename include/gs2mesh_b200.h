@@ -392,6 +392,29 @@ int gsb_eval_cull_vertices_by_masks(const double* vertices, int64_t n_vertices, 
                                     int32_t image_width, int32_t image_height, int32_t mask_width, int32_t mask_height,
                                     const uint32_t* packed_masks, uint8_t* keep, void* stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Stereo stage (gs2mesh_utils/stereo_utils.py:82-179) around the caller's disparity model.
+ * ------------------------------------------------------------------------------------------
+ * Frames are width x height with 1 <= width <= GSB_TSDF_MAX_WIDTH, 1 <= height <= GSB_TSDF_MAX_HEIGHT.  The model's
+ * inputs are padded like DLNR's InputPadder(dims, divis_by=32) ('sintel'): ph = ((H/32 + 1)*32 - H) % 32 (pw likewise),
+ * [l, r, t, b] = [pw/2, pw - pw/2, ph/2, ph - ph/2], Hp = H + t + b, Wp = W + l + r.
+ *   gsb_stereo_pack_inputs      left / right: device uint8 [H,W,3]; out: device float [4,3,Hp,Wp] =
+ *                               pad(left), pad(right), flip_x(pad(right)), flip_x(pad(left)), replicate padding, float(u8).
+ *   gsb_stereo_disparities      flow_lr / flow_rl: the model's full-resolution outputs, device float [Hp,Wp];
+ *                               disp_lr[y][x] = sign * flow_lr[t+y][l+x] (device float [H,W]),
+ *                               disp_rl[y][x] = sign * flow_rl[y][Wp-1-x] (device float [Hp,Wp], not cropped).
+ *                               Outputs must not alias the inputs.
+ *   gsb_stereo_occlusion_depth  get_occlusion_mask(disp_lr, disp_rl, threshold) and depth = fx*B / disp_lr per pixel, in
+ *                               numpy's dtypes (DESIGN.md section 7c): visible (device uint8 [H,W], 1 = visible) reads row y,
+ *                               column xc of disp_rl with row stride rl_stride >= width (elements); depth (device float
+ *                               [H,W]) = depth_numerator / disp_lr in fp32, depth_numerator = float(fx * B) rounded once on
+ *                               the host.  Either output may be NULL (not both); disp_rl may be NULL when visible is. */
+int gsb_stereo_pack_inputs(const uint8_t* left, const uint8_t* right, int32_t width, int32_t height, float* out, void* stream);
+int gsb_stereo_disparities(const float* flow_lr, const float* flow_rl, int32_t width, int32_t height, float sign, float* disp_lr,
+                           float* disp_rl, void* stream);
+int gsb_stereo_occlusion_depth(const float* disp_lr, const float* disp_rl, int32_t width, int32_t height, int64_t rl_stride,
+                               double threshold, float depth_numerator, uint8_t* visible, float* depth, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
