@@ -143,13 +143,14 @@ __global__ void __launch_bounds__(256) grid_scatter_kernel(const GsbPointGrid g,
 
 // Rings of cells at Chebyshev distance k around the query's (unclamped) cell.  Every point in a ring > k lies at least
 // k*h away, so the search stops once the best distance is below that bound (with a relative margin far above the
-// rounding error of the distance expression), or once k*h reaches max_dist.
-__global__ void __launch_bounds__(128) nearest_kernel(const GsbPointGrid g, const double* __restrict__ q, long long nq,
-                                                      double max_dist, double* __restrict__ out_dist,
-                                                      long long* __restrict__ out_idx) {
-  const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (t >= nq) return;
-  const double qx = q[3 * t], qy = q[3 * t + 1], qz = q[3 * t + 2];
+// rounding error of the distance expression), or once k*h reaches max_dist.  Returns the nearest point (lowest index
+// among equal squared distances; -1 if none) and its ((dx*dx)+dy*dy)+dz*dz; a point at max_dist or beyond may be missed.
+struct Nearest {
+  double d2;
+  long long id;
+};
+
+__device__ __forceinline__ Nearest ring_nearest(const GsbPointGrid& g, double qx, double qy, double qz, double max_dist) {
   const long long qc[3] = {(long long)floor((qx - g.origin[0]) / g.cell), (long long)floor((qy - g.origin[1]) / g.cell),
                            (long long)floor((qz - g.origin[2]) / g.cell)};
   // first ring that can reach the grid, last ring that still meets it
@@ -193,10 +194,32 @@ __global__ void __launch_bounds__(128) nearest_kernel(const GsbPointGrid g, cons
       }
     }
   }
-  const double d = best >= 0 ? __dsqrt_rn(best2) : INFINITY;
+  return {best2, best};
+}
+
+__global__ void __launch_bounds__(128) nearest_kernel(const GsbPointGrid g, const double* __restrict__ q, long long nq,
+                                                      double max_dist, double* __restrict__ out_dist,
+                                                      long long* __restrict__ out_idx) {
+  const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= nq) return;
+  const Nearest nb = ring_nearest(g, q[3 * t], q[3 * t + 1], q[3 * t + 2], max_dist);
+  const double d = nb.id >= 0 ? __dsqrt_rn(nb.d2) : INFINITY;
   const bool hit = d < max_dist;
   out_dist[t] = hit ? d : INFINITY;
-  out_idx[t] = hit ? best : -1;
+  out_idx[t] = hit ? nb.id : -1;
+}
+
+// ICP correspondences (Open3D's KDTreeFlann::SearchHybrid(p, r, 1) over nanoflann): the nearest target point with
+// ((dx*dx)+dy*dy)+dz*dz < r*r, strictly on the squared distance; misses get (-1, +inf).
+__global__ void __launch_bounds__(128) icp_correspond_kernel(const GsbPointGrid g, const double* __restrict__ q, long long nq,
+                                                             double r, double r2, long long* __restrict__ out_idx,
+                                                             double* __restrict__ out_d2) {
+  const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= nq) return;
+  const Nearest nb = ring_nearest(g, q[3 * t], q[3 * t + 1], q[3 * t + 2], r);
+  const bool hit = nb.id >= 0 && nb.d2 < r2;
+  out_idx[t] = hit ? nb.id : -1;
+  out_d2[t] = hit ? nb.d2 : INFINITY;
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -343,6 +366,19 @@ int gsb_eval_nearest(const GsbPointGrid* grid, const double* queries, int64_t n_
                                                                           reinterpret_cast<long long*>(index));
   count_launch();
   return check_launch("nearest_kernel", stream, false);
+}
+
+int gsb_eval_icp_correspond(const GsbPointGrid* grid, const double* source, int64_t n_source, double radius, int64_t* index,
+                            double* dist2, void* stream_v) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
+  if (!grid_ok(grid) || (grid->n_points && !grid->ids) || n_source < 0 || (n_source && (!source || !index || !dist2)) ||
+      !(radius > 0.0) || !(radius < INFINITY))
+    return fail(GSB_ERR_INVALID, "eval_icp_correspond: bad arguments");
+  if (n_source == 0) return GSB_OK;
+  icp_correspond_kernel<<<(unsigned)((n_source + 127) / 128), 128, 0, stream>>>(*grid, source, n_source, radius, radius * radius,
+                                                                                reinterpret_cast<long long*>(index), dist2);
+  count_launch();
+  return check_launch("icp_correspond_kernel", stream, false);
 }
 
 int gsb_eval_radius_downsample(const GsbPointGrid* grid, double radius, uint8_t* keep, uint32_t* counters,

@@ -377,6 +377,45 @@ int gsb_eval_nearest(const GsbPointGrid* grid, const double* queries, int64_t n_
 int gsb_eval_radius_downsample(const GsbPointGrid* grid, double radius, uint8_t* keep, uint32_t* counters,
                                uint32_t* host_undecided, int32_t* rounds, void* stream);
 
+/* Tanks and Temples evaluation (evaluation/TNT/eval_code/python_toolbox/evaluation), restating Open3D 0.17's
+ * PointCloud::Transform, SelectionPolygonVolume::CropInPolygon, VoxelDownSample and RegistrationICP with
+ * TransformationEstimationPointToPoint (Eigen::umeyama); DESIGN.md section 7d gives each operation order.
+ *   gsb_eval_transform_points  out[i] = (T (p_i, 1)).xyz / (T (p_i, 1)).w, rows ((T_r0*x + T_r1*y) + T_r2*z) + T_r3.
+ *                              transform: host double [4][4] row-major.  out may equal points.
+ *   gsb_eval_crop_polygon      keep[i] = 1 iff axis_min <= p_w <= axis_max and p lies inside the polygon (odd count of edge
+ *                              crossings below p_u); orthogonal_axis 0/1/2 = x/y/z picks (u, v, w) = (1,2,0)/(0,2,1)/(0,1,2).
+ *                              polygon: device double [n_vertices,3], 3 <= n_vertices <= GSB_EVAL_MAX_POLYGON.
+ *                              counter: device uint32 scratch; host_non_finite: pinned host uint32.  SYNCHRONISES the
+ *                              stream and returns GSB_ERR_INVALID when a point is not finite.
+ *   gsb_eval_voxel_downsample  the mean of the points of each voxel floor((p - lo) / voxel_size), lo = min_bound -
+ *                              voxel_size/2, summed in input order, one output point per voxel in ascending (x, y, z)
+ *                              voxel order.  min_bound / max_bound: host double [3], the points' bounds.  out: device
+ *                              double [n_points,3]; n_out: device int64, the number of voxels.  GSB_ERR_INVALID when
+ *                              voxel_size * INT_MAX < the padded extent (Open3D's "voxel_size is too small") or when the
+ *                              voxel keys need more than 63 bits.  n_points < 2^31.
+ *   gsb_eval_icp_correspond    index[i] = the nearest grid point with ((dx*dx)+dy*dy)+dz*dz < radius*radius, else -1;
+ *                              dist2[i] its squared distance (+inf for -1).
+ *   gsb_eval_icp_moments       sums over the correspondences (index[i] >= 0) with a fixed reduction tree (the same bits on
+ *                              every run): pass 0 writes out[0..6] = (sum dist2, sum source xyz, sum target[index] xyz);
+ *                              pass 1, given means = host double [6] (source mean, target mean), writes out[0..8] =
+ *                              sum (t - mu_t)_j (s - mu_s)_k (j-major) and out[9..11] = sum (s - mu_s)_k^2.  out[12] =
+ *                              the number of correspondences.  out: device double [13]; workspace: device double
+ *                              [GSB_EVAL_ICP_MOMENT_WORKSPACE]. */
+#define GSB_EVAL_MAX_POLYGON 2048
+#define GSB_EVAL_ICP_MOMENT_WORKSPACE (13 * 256)
+int gsb_eval_transform_points(const double* points, int64_t n_points, const double* transform, double* out, void* stream);
+int gsb_eval_crop_polygon(const double* points, int64_t n_points, const double* polygon, int32_t n_vertices,
+                          int32_t orthogonal_axis, double axis_min, double axis_max, uint8_t* keep, uint32_t* counter,
+                          uint32_t* host_non_finite, void* stream);
+size_t gsb_eval_voxel_workspace_bytes(int64_t n_points);
+int gsb_eval_voxel_downsample(const double* points, int64_t n_points, const double* min_bound, const double* max_bound,
+                              double voxel_size, void* workspace, size_t workspace_bytes, double* out, int64_t* n_out,
+                              void* stream);
+int gsb_eval_icp_correspond(const GsbPointGrid* grid, const double* source, int64_t n_source, double radius, int64_t* index,
+                            double* dist2, void* stream);
+int gsb_eval_icp_moments(const double* source, const int64_t* index, const double* dist2, int64_t n_source,
+                         const double* target, int pass, const double* means, double* workspace, double* out, void* stream);
+
 /* Mesh culling by object masks (evaluation/DTU/eval_code/evaluate_single_scene.py:21-116, `cull_scan`).
  * Binary dilation of n_views masks (device uint8 [n_views,height,width], nonzero = set) by the disk x*x + y*y <= r*r
  * (skimage disk(r)); pixels outside the image are unset.  packed: device uint32 [n_views][height][(width+31)/32], pixel x
