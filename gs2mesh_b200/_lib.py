@@ -20,18 +20,6 @@ RASTER_CUB_SORT = 8
 RASTER_ASYNC = 16
 RASTER_FAST_EXP = 32
 RASTER_PAIR_SHARED_DEPTH = 64
-RENDER_IMPLS = {"dual": 4, "table": 5}
-SH_MODES = {"scalar": 1, "vec": 2, "padded": 3}
-
-
-def RASTER_RENDER_IMPL(name_or_n):
-    """flags field selecting the blend kernel variant (include/gs2mesh_b200.h: GSB_RASTER_RENDER_IMPL)."""
-    return (int(RENDER_IMPLS.get(name_or_n, name_or_n)) & 7) << 8
-
-
-def RASTER_SH_MODE(name_or_n):
-    """flags field selecting the SH staging variant (GSB_RASTER_SH_MODE)."""
-    return (int(SH_MODES.get(name_or_n, name_or_n)) & 3) << 12
 
 BRICK = 16
 BRICK_VOXELS = 4096

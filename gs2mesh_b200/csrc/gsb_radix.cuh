@@ -13,8 +13,6 @@
 // memory and written out in runs.
 #pragma once
 
-#include <cstdlib>
-
 #include "gsb_common.h"
 
 namespace gsb {
@@ -27,10 +25,8 @@ constexpr int kRdxBlock = kRdxThreads * kRdxItems;     // 4096 items per CTA
 constexpr int kRdxBins = 256;
 constexpr int kRdxMaxPasses = 4;
 constexpr int kRdxWindow = 8;                          // predecessors inspected per look-back round
-constexpr int kRdxDefaultPItems = 8;                   // items per thread of small sorts; GSB_RADIX_P_ITEMS overrides
+constexpr int kRdxSmallItems = 8;                      // items per thread of small sorts
 constexpr size_t kRdxSmallSort = 1u << 22;             // sorts of up to 4M items count as "small" (the P-sized depth sort)
-constexpr int kRdxDefaultEvenSplit = 1;                // GSB_RADIX_SPLIT=even|byte overrides (A/B switch)
-constexpr int kRdxDefaultWindowed = 1;                 // GSB_RADIX_LOOKBACK=serial|window overrides (A/B switch)
 
 // status word of (block, digit): [31:30] 0 = not ready, 1 = block aggregate, 2 = inclusive prefix
 constexpr uint32_t kStAgg = 1u << 30, kStIncl = 2u << 30, kStVal = (1u << 30) - 1u;
@@ -107,9 +103,9 @@ __device__ __forceinline__ void st_status(uint32_t* p, uint32_t v) {
 // pass of the tile sort: keys are then fully sorted tile ids and the first / last instance of every
 // tile seen by the block updates ranges[tile] = (start, end) with atomicMin / atomicMax.
 // kItems = items per thread: 16 for the R-sized instance sorts; the P-sized depth sort, whose whole grid is co-resident
-// and therefore runs at the latency of ONE block, may use smaller blocks (more, shorter critical paths).
+// and therefore runs at the latency of ONE block, uses 8 (more, shorter critical paths).
 template <int kItems>
-__global__ void __launch_bounds__(kRdxThreads, kItems >= 16 ? 3 : (kItems >= 8 ? 4 : 5)) radix_pass_kernel(const uint32_t* __restrict__ keys_in,
+__global__ void __launch_bounds__(kRdxThreads, kItems >= 16 ? 3 : 4) radix_pass_kernel(const uint32_t* __restrict__ keys_in,
                                                                 const uint32_t* __restrict__ vals_in,
                                                                 uint32_t* __restrict__ keys_out,
                                                                 uint32_t* __restrict__ vals_out, uint32_t n_host,
@@ -117,7 +113,7 @@ __global__ void __launch_bounds__(kRdxThreads, kItems >= 16 ? 3 : (kItems >= 8 ?
                                                                 int64_t capacity, int shift, uint32_t dmask,
                                                                 const uint32_t* __restrict__ ghist,
                                                                 uint32_t* __restrict__ status, uint32_t* __restrict__ ticket,
-                                                                uint2* __restrict__ ranges, int window, int write_keys,
+                                                                uint2* __restrict__ ranges, int write_keys,
                                                                 const uint32_t* __restrict__ gather_src,
                                                                 uint32_t* __restrict__ gather_dst,
                                                                 const uint32_t* __restrict__ gather_src2,
@@ -199,40 +195,27 @@ __global__ void __launch_bounds__(kRdxThreads, kItems >= 16 ? 3 : (kItems >= 8 ?
     st_status(my, (bid == 0 ? kStIncl : kStAgg) | run);
     uint32_t prev = 0;
     if (bid > 0) {
-      if (window <= 1) {
-        for (int64_t b = (int64_t)bid - 1; b >= 0; --b) {
-          const uint32_t* sp = status + (size_t)b * kRdxBins + d;
-          uint32_t sv = ld_status(sp);
-          for (uint32_t spin = 0; (sv >> 30) == 0; ++spin) {
-            if (spin > (1u << 24)) __trap();  // a predecessor never published: fail loudly instead of hanging
-            sv = ld_status(sp);
-          }
-          prev += sv & kStVal;
-          if ((sv >> 30) == 2) break;
-        }
-      } else {
-        // Windowed look-back: the status words of kRdxWindow predecessors are requested at once (independent
-        // loads), then consumed newest-first.  When every block of a pass starts at the same time (the whole
-        // P-sized grid is co-resident) a one-word-at-a-time walk costs ~nblocks/2 dependent L2 round trips;
-        // this cuts the chain by the window length.  Every word is self-contained (flag + count), so a
-        // speculative read of an older word is valid whatever state the newer ones were in.
-        bool closed = false;
-        for (int64_t b = (int64_t)bid - 1; !closed; b -= kRdxWindow) {
-          uint32_t sv[kRdxWindow];
+      // Windowed look-back: the status words of kRdxWindow predecessors are requested at once (independent
+      // loads), then consumed newest-first.  When every block of a pass starts at the same time (the whole
+      // P-sized grid is co-resident) a one-word-at-a-time walk costs ~nblocks/2 dependent L2 round trips;
+      // this cuts the chain by the window length.  Every word is self-contained (flag + count), so a
+      // speculative read of an older word is valid whatever state the newer ones were in.
+      bool closed = false;
+      for (int64_t b = (int64_t)bid - 1; !closed; b -= kRdxWindow) {
+        uint32_t sv[kRdxWindow];
 #pragma unroll
-          for (int j = 0; j < kRdxWindow; ++j)
-            sv[j] = b - j >= 0 ? ld_status(status + (size_t)(b - j) * kRdxBins + d) : kStIncl;  // before block 0: prefix 0
+        for (int j = 0; j < kRdxWindow; ++j)
+          sv[j] = b - j >= 0 ? ld_status(status + (size_t)(b - j) * kRdxBins + d) : kStIncl;  // before block 0: prefix 0
 #pragma unroll
-          for (int j = 0; j < kRdxWindow; ++j) {
-            if (!closed) {
-              uint32_t v = sv[j];
-              for (uint32_t spin = 0; (v >> 30) == 0; ++spin) {
-                if (spin > (1u << 24)) __trap();  // a predecessor never published: fail loudly instead of hanging
-                v = ld_status(status + (size_t)(b - j) * kRdxBins + d);
-              }
-              prev += v & kStVal;
-              closed = (v >> 30) == 2;
+        for (int j = 0; j < kRdxWindow; ++j) {
+          if (!closed) {
+            uint32_t v = sv[j];
+            for (uint32_t spin = 0; (v >> 30) == 0; ++spin) {
+              if (spin > (1u << 24)) __trap();  // a predecessor never published: fail loudly instead of hanging
+              v = ld_status(status + (size_t)(b - j) * kRdxBins + d);
             }
+            prev += v & kStVal;
+            closed = (v >> 30) == 2;
           }
         }
       }
@@ -302,49 +285,22 @@ __global__ void __launch_bounds__(kRdxThreads, kItems >= 16 ? 3 : (kItems >= 8 ?
   }
 }
 
-inline int radix_lookback_window() {
-  static const int w = [] {
-    const char* e = getenv("GSB_RADIX_LOOKBACK");
-    if (e && e[0] == 's') return 1;
-    if (e && e[0] == 'w') return kRdxWindow;
-    return kRdxDefaultWindowed ? kRdxWindow : 1;
-  }();
-  return w;
-}
-
 // Items per thread of a sort over at most `max_items` items.
-inline int radix_items_for(size_t max_items) {
-  static const int p_items = [] {
-    const char* e = getenv("GSB_RADIX_P_ITEMS");  // A/B switch: 4 | 8 | 16
-    const int v = e ? atoi(e) : kRdxDefaultPItems;
-    return (v == 4 || v == 8) ? v : 16;
-  }();
-  static const int r_items = [] {
-    const char* e = getenv("GSB_RADIX_R_ITEMS");  // A/B switch for the instance sorts: 4 | 8 | 16
-    const int v = e ? atoi(e) : kRdxItems;
-    return (v == 4 || v == 8) ? v : 16;
-  }();
-  return max_items <= kRdxSmallSort ? p_items : r_items;
-}
+inline int radix_items_for(size_t max_items) { return max_items <= kRdxSmallSort ? kRdxSmallItems : kRdxItems; }
 inline size_t radix_blocks_for(size_t max_items) {
   const size_t block = (size_t)kRdxThreads * radix_items_for(max_items);
   return (max_items + block - 1) / block;
 }
 
 // Bits per digit of a sort over `bits` key bits: the passes share the bits evenly (13 tile-id bits -> 7 + 6 instead
-// of 8 + 5: fewer, longer same-digit runs per block in the first pass).  GSB_RADIX_SPLIT=byte restores 8-bit digits.
+// of 8 + 5: fewer, longer same-digit runs per block in the first pass).
 inline int radix_digit_bits(int bits) {
-  static const int even = [] {
-    const char* e = getenv("GSB_RADIX_SPLIT");
-    if (e && e[0] == 'b') return 0;
-    if (e && e[0] == 'e') return 1;
-    return kRdxDefaultEvenSplit;
-  }();
   const int passes = (bits + 7) / 8;
-  return even ? (bits + passes - 1) / passes : 8;
+  return (bits + passes - 1) / passes;
 }
 
-// Scratch words one sort needs for `max_items` items (sized for the smallest block either sort may use).
+// Scratch words one sort needs for `max_items` items.  Sized for blocks of 4 items per thread, half the smallest block
+// either sort uses: a margin that keeps every gsb_raster_workspace_bytes value as it was.
 inline size_t radix_scratch_words(size_t max_items) {
   const size_t nblocks = (max_items + kRdxThreads * 4 - 1) / (kRdxThreads * 4);
   return (size_t)kRdxMaxPasses * (kRdxBins + nblocks * kRdxBins + 1) + 64;
@@ -394,7 +350,7 @@ inline int radix_sort_pairs_t(uint32_t* keys_a, uint32_t* vals_a, uint32_t* keys
     radix_pass_kernel<kItems><<<nblocks, kRdxThreads, 0, stream>>>(
         kin, vin, kout, vout, n_host, counters, capacity, db * p, (1u << db) - 1u, ghist + p * kRdxBins,
         status + (size_t)p * nblocks * kRdxBins,
-        tickets + p, p == passes - 1 ? ranges_on_last_pass : nullptr, radix_lookback_window(), p != passes - 1,
+        tickets + p, p == passes - 1 ? ranges_on_last_pass : nullptr, p != passes - 1,
         gather_src, p == passes - 1 ? gather_dst : nullptr, gather_src2, p == passes - 1 ? gather_dst2 : nullptr);
     *launches += 1;
     cur ^= 1;
@@ -408,16 +364,9 @@ inline int radix_sort_pairs(uint32_t* keys_a, uint32_t* vals_a, uint32_t* keys_b
                             bool histogram_ready, const uint32_t* gather_src = nullptr, uint32_t* gather_dst = nullptr,
                             const uint32_t* gather_src2 = nullptr, uint32_t* gather_dst2 = nullptr,
                             bool identity_payload = false) {
-#define GSB_RADIX_CALL(ITEMS)                                                                                              \
-  radix_sort_pairs_t<ITEMS>(keys_a, vals_a, keys_b, vals_b, n_host, counters, capacity, max_items, bits, scratch,          \
-                            ranges_on_last_pass, stream, launches, histogram_ready, gather_src, gather_dst, gather_src2,   \
-                            gather_dst2, identity_payload)
-  switch (radix_items_for(max_items)) {
-    case 4: return GSB_RADIX_CALL(4);
-    case 8: return GSB_RADIX_CALL(8);
-    default: return GSB_RADIX_CALL(16);
-  }
-#undef GSB_RADIX_CALL
+  const auto sort = radix_items_for(max_items) == kRdxSmallItems ? radix_sort_pairs_t<kRdxSmallItems> : radix_sort_pairs_t<kRdxItems>;
+  return sort(keys_a, vals_a, keys_b, vals_b, n_host, counters, capacity, max_items, bits, scratch, ranges_on_last_pass, stream,
+              launches, histogram_ready, gather_src, gather_dst, gather_src2, gather_dst2, identity_payload);
 }
 
 }  // namespace

@@ -29,7 +29,6 @@
 //
 // All kernels run on the caller's stream(s).
 #include <algorithm>
-#include <cstdlib>
 
 #include <cub/cub.cuh>
 
@@ -396,17 +395,13 @@ struct PreParams {
   uint32_t gx, gy;
   uint32_t flags;
   int use_tma;
-  int sh_mode;  // staging of full-degree SH blocks (M = 16): 0 linear + scalar reads, 1 linear + 16-byte reads,
-                // 2 one 192-byte bulk copy per lane into padded slots + 16-byte reads (bank-conflict free)
   int binned;        // 0: validation path (no depth keys, no tile masks)
   int shared_depth;  // stereo pair whose eyes see every Gaussian at the same view depth: one key array (eye 0's), verified
   PreEye eye[2];
 };
 
-constexpr int kDefaultShMode = 1;                // GSB_PRE_SH overrides (A/B switch)
-constexpr int kShPadStride = kMaxShFloats + 4;  // 208-byte slots: 16-byte reads of 32 lanes hit distinct banks
 struct WarpStage {  // one warp's staged parameter block; every member offset is a multiple of 128 B
-  float sh[32 * kShPadStride];  // 6656 B
+  float sh[32 * (kMaxShFloats + 4)];  // 6656 B, 512 B more than the SH block: the 8 KB stage the kernels were timed with
   float rot[32 * 4];            // 512 B
   float xyz[32 * 3];            // 384 B
   float scale[32 * 3];          // 384 B
@@ -612,16 +607,11 @@ __global__ void __launch_bounds__(kPreThreads, kMinBlocks) preprocess_kernel(con
   const int shf = p.M * 3;  // SH floats per Gaussian
   const bool need_sh = p.colors == nullptr && any_visible;
   const bool tma_sh = need_sh && full_tma && (shf * 4) % 16 == 0 && shf <= kMaxShFloats;
-  const int sh_mode = shf == kMaxShFloats ? p.sh_mode : 0;
-  const int sh_stride = sh_mode == 2 ? kShPadStride : shf;
-  if (tma_sh) {
-    if (lane == 0) mbar_expect_tx(&st.bar, (uint32_t)(32 * shf * 4));
-    if (sh_mode == 2) {
-      __syncwarp();  // the transaction count is armed before any lane's copy can complete
-      tma_load_1d(st.sh + lane * kShPadStride, p.shs + (size_t)(base + lane) * shf, (uint32_t)(shf * 4), &st.bar);
-    } else if (lane == 0) {
-      tma_load_1d(st.sh, p.shs + (size_t)base * shf, (uint32_t)(32 * shf * 4), &st.bar);
-    }
+  // full-degree blocks (M = 16, 192 B per lane) are read as 16-byte vectors; smaller ones as scalars
+  const bool vec_sh = shf == kMaxShFloats;
+  if (tma_sh && lane == 0) {
+    mbar_expect_tx(&st.bar, (uint32_t)(32 * shf * 4));
+    tma_load_1d(st.sh, p.shs + (size_t)base * shf, (uint32_t)(32 * shf * 4), &st.bar);
   }
   // binning, pass 1: how many tiles this Gaussian is binned into.  The staged rotations / positions / scales are dead by
   // now: their 1280 bytes carry the lanes' footprints during binning (32 x 2 float4 = 1024 bytes)
@@ -646,13 +636,13 @@ __global__ void __launch_bounds__(kPreThreads, kMinBlocks) preprocess_kernel(con
       if (tma_sh) {
         mbar_wait(&st.bar, 1);
       } else {
-        for (int k = lane; k < count * shf; k += 32) st.sh[(k / shf) * sh_stride + k % shf] = p.shs[(size_t)base * shf + k];
+        for (int k = lane; k < count * shf; k += 32) st.sh[k] = p.shs[(size_t)base * shf + k];
         __syncwarp();
       }
       if (vis_any) {
-        const float* sh = st.sh + lane * sh_stride;
+        const float* sh = st.sh + lane * shf;
         float shreg[kMaxShFloats];
-        if (sh_mode != 0) {  // 12 x 16-byte reads, then the arithmetic from registers (both eyes share the reads)
+        if (vec_sh) {  // 12 x 16-byte reads, then the arithmetic from registers (both eyes share the reads)
           const float4* s4 = reinterpret_cast<const float4*>(sh);
 #pragma unroll
           for (int k = 0; k < kMaxShFloats / 4; ++k) {
@@ -674,7 +664,7 @@ __global__ void __launch_bounds__(kPreThreads, kMinBlocks) preprocess_kernel(con
           dir.y = dir.y / len;
           dir.z = dir.z / len;
           float res[3];
-          if (sh_mode != 0)
+          if (vec_sh)
             eval_sh(p.D, [&](int i) { return shreg[i]; }, dir, res);
           else
             eval_sh(p.D, [&](int i) { return sh[i]; }, dir, res);
@@ -1063,15 +1053,10 @@ __device__ __forceinline__ void sts64(uint32_t addr, const float2& v) {
   asm volatile("st.shared.v2.f32 [%0], {%1,%2};" ::"r"(addr), "f"(v.x), "f"(v.y) : "memory");
 }
 
-__device__ __forceinline__ float ex2_ftz(float x) {
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
-
-// forward.cu:261-374, re-organised ("dual" kernel: the blend with the reference's own exponent expression, full-precision
-// expf or ex2.approx; the default table kernel below restructures the exponent).  Per 16x16 tile four warps that never
-// wait for each other: every warp streams the tile's sorted instance list on its own, 32 Gaussians at a time -- each lane
+// forward.cu:261-374, re-organised: the blend without GSB_RASTER_FAST_EXP, with the reference's own exponent expression
+// and full-precision expf (transmittance bit-identical to the reference's; the default table kernel below restructures
+// the exponent).  Per 16x16 tile four warps that never wait for each other: every warp streams the tile's sorted
+// instance list on its own, 32 Gaussians at a time -- each lane
 // gathers ONE record (the warps of the CTA hit the same lines, so all but the first gather is an L1 hit) and tests it
 // against the warp's 8x8 pixel block with the exact footprint test straight from registers.  The lanes whose Gaussian
 // passed store their record at consecutive 48-byte slots (ballot rank) of the warp's private double-buffered list, so the
@@ -1081,13 +1066,12 @@ __device__ __forceinline__ float ex2_ftz(float x) {
 // per trip.  The next chunk's gathers are in flight while the current one is blended; a warp leaves as soon as its own 64
 // pixels are saturated.  Skipped Gaussians are exactly the ones every pixel of the block would `continue` past in the
 // reference loop; colours accumulate as fma(c, alpha*T, C) (the reference: fma(c*alpha, T, C), <= 1 ulp per term).
-constexpr int kDefaultRenderImpl = 4;        // 3 dual, 4 table (GSB_RENDER_IMPL overrides)
 constexpr int kSlotBytes = 48;               // A (16) | B (16) | green, blue (8) | pad (8)
 constexpr int kSlotsPerBuf = 33;             // 32 hits + sentinel
-// kPix = pixels per lane: 1 -> 8 warps per tile, each an 8x4 block; 2 -> 4 warps per tile, each an 8x8 block whose
-// lanes own (x, y) and (x, y + 4): the list walk, the footprint test and the record loads are shared by 64 pixels.
-template <bool kFastExp, int kPix>
-__global__ void __launch_bounds__(kTilePixels / kPix, kPix == 1 ? 5 : 8)
+// kPix = 2 pixels per lane: 4 warps per tile, each an 8x8 block whose lanes own (x, y) and (x, y + 4): the list walk,
+// the footprint test and the record loads are shared by 64 pixels.
+constexpr int kPix = 2;
+__global__ void __launch_bounds__(kTilePixels / kPix, 8)
     render_compact_kernel(const uint2* __restrict__ ranges, const uint32_t* __restrict__ point_list, int W, int H,
                           const float4* __restrict__ recA, const float4* __restrict__ recB, const float2* __restrict__ recC,
                           const float* __restrict__ bg, float* __restrict__ out_color, float* __restrict__ out_depth,
@@ -1133,8 +1117,7 @@ __global__ void __launch_bounds__(kTilePixels / kPix, kPix == 1 ? 5 : 8)
     for (int k = 0; k < kPix; ++k) {
       const float dy = A.y - pfy[k];
       const float power = -0.5f * (B.x * dx * dx + B.z * dy * dy) - B.y * dx * dy;
-      const float e = kFastExp ? ex2_ftz(power * 1.4426950408889634f) : exp(power);
-      const float alpha = min(0.99f, A.w * e);
+      const float alpha = min(0.99f, A.w * exp(power));
       const float test_T = T[k] * (1 - alpha);
       const bool cand = !done[k] && !(power > 0.0f) && !(alpha < 1.0f / 255.0f);
       const bool sat = cand && test_T < 0.0001f;
@@ -1205,8 +1188,9 @@ __global__ void __launch_bounds__(kTilePixels / kPix, kPix == 1 ? 5 : 8)
 }
 
 // ---------------------------------------------------------------------------------------------
-// Table variant of render_compact_kernel<true, 2> (default): same per-warp compacted hit list, but the blend loop is
-// cut from 29 to ~16 issue slots per (record, pixel) by moving everything that does not depend on the pixel out of it.
+// Table kernel (the GSB_RASTER_FAST_EXP blend, default): render_compact_kernel's per-warp compacted hit list, but the blend
+// loop -- 29 issue slots per (record, pixel) in that kernel's shape with ex2.approx -- is cut to ~16 by moving everything
+// that does not depend on the pixel out of it.
 // FSETP / FSEL / FMNMX issue on the ALU pipe, which has half the FMA pipe's rate, and MUFU.EX2 is slower still.  Here:
 //  * the exponent is evaluated in the log2 domain as  e = u'(x) + v(x)*dy(y) + w(y)  with
 //        u'(x) = -0.5 log2e a dx^2 + log2(opacity),  v(x) = -log2e b dx,  w(y) = -0.5 log2e c dy^2 ;
@@ -1664,6 +1648,9 @@ static cudaEvent_t pair_event() {
   return e;
 }
 
+constexpr uint32_t kRasterFlags = GSB_RASTER_EXACT_TILE_CULL | GSB_RASTER_NO_TMA | GSB_RASTER_DEBUG_SYNC | GSB_RASTER_CUB_SORT |
+                                  GSB_RASTER_FAST_EXP | GSB_RASTER_PAIR_SHARED_DEPTH | GSB_RASTER_ASYNC;
+
 static int validate_frame(const GsbRasterArgs* a, Frame& f) {
   if (!a) return fail(GSB_ERR_INVALID, "args is NULL");
   if (a->P < 0 || a->width <= 0 || a->height <= 0) return fail(GSB_ERR_INVALID, "bad P / image size");
@@ -1682,7 +1669,10 @@ static int validate_frame(const GsbRasterArgs* a, Frame& f) {
                  (a->sh_degree + 1) * (a->sh_degree + 1) > a->sh_coeffs))
     return fail(GSB_ERR_INVALID, "SH degree %d needs %d coefficients, tensor has %d (max 16)", a->sh_degree,
                 (a->sh_degree + 1) * (a->sh_degree + 1), a->sh_coeffs);
-  if (!a->workspace) return fail(GSB_ERR_WORKSPACE, "workspace is NULL");
+  if (a->flags & ~kRasterFlags)
+    return fail(GSB_ERR_INVALID, "flags 0x%x: undefined bits 0x%x (not a GSB_RASTER_* flag)", (unsigned)a->flags,
+                (unsigned)(a->flags & ~kRasterFlags));
+  if (!a->workspace)return fail(GSB_ERR_WORKSPACE, "workspace is NULL");
   if (a->max_instances >= (int64_t)kStVal)  // the emit pass's scan words hold 30-bit instance counts
     return fail(GSB_ERR_INVALID, "max_instances must be below 2^30 - 1");
   f.a = a;
@@ -1729,14 +1719,6 @@ static void fill_common(const Frame& f, PreParams& pp) {
   pp.flags = a->flags;
   pp.use_tma = !(a->flags & GSB_RASTER_NO_TMA) && aligned16(a->means3D) && aligned16(a->opacities) &&
                (!has_sr || (aligned16(a->scales) && aligned16(a->rotations))) && (!a->shs || aligned16(a->shs));
-  static const int sh_mode_default = [] {
-    const char* e = getenv("GSB_PRE_SH");  // A/B switch: "scalar" | "vec" | "padded"
-    if (e && e[0] == 's') return 0;
-    if (e && e[0] == 'v') return 1;
-    if (e && e[0] == 'p') return 2;
-    return kDefaultShMode;
-  }();
-  pp.sh_mode = ((a->flags >> 12) & 3u) ? (int)((a->flags >> 12) & 3u) - 1 : sh_mode_default;
 }
 
 static void fill_eye(const Frame& f, PreEye& e) {
@@ -1830,29 +1812,17 @@ static int render_frame_impl(const Frame& f, const uint32_t* point_list, cudaStr
   const uint32_t gx = f.gx, gy = f.gy;
   {
     StageTimer tm(kStRender, stream);
-    static const int render_impl = [] {  // A/B switch for profiling: "dual" | "table"
-      const char* e = getenv("GSB_RENDER_IMPL");
-      if (e && e[0] == 'd') return 3;
-      if (e && e[0] == 't') return 4;
-      return kDefaultRenderImpl;
-    }();
-    const int impl = ((a->flags >> 8) & 7u) ? (int)((a->flags >> 8) & 7u) - 1 : render_impl;
-    const bool fast = (a->flags & GSB_RASTER_FAST_EXP) != 0;
-#define GSB_LAUNCH_RENDER_T(THREADS, ...)                                                                                \
-  __VA_ARGS__<<<dim3(gx, gy), THREADS, 0, stream>>>(ws.ranges, point_list, W, H, ws.recA, ws.recB, ws.recC, a->background, \
-                                                    a->out_color, a->out_depth, a->out_final_T, cap)
-    if (impl == 4 && fast) {
-      if (g_blend_trace_on.load()) {
-        GSB_LAUNCH_RENDER_T(kTilePixels / 2, render_table_kernel<true>);
-      } else {
-        GSB_LAUNCH_RENDER_T(kTilePixels / 2, render_table_kernel<false>);
-      }
-    } else if (fast) {  // the table kernel only exists for the ex2 blend: full-precision expf -> dual
-      GSB_LAUNCH_RENDER_T(kTilePixels / 2, render_compact_kernel<true, 2>);
+#define GSB_LAUNCH_RENDER(KERNEL)                                                                                         \
+  KERNEL<<<dim3(gx, gy), kTilePixels / 2, 0, stream>>>(ws.ranges, point_list, W, H, ws.recA, ws.recB, ws.recC, a->background, \
+                                                       a->out_color, a->out_depth, a->out_final_T, cap)
+    if (!(a->flags & GSB_RASTER_FAST_EXP)) {
+      GSB_LAUNCH_RENDER(render_compact_kernel);
+    } else if (g_blend_trace_on.load()) {
+      GSB_LAUNCH_RENDER(render_table_kernel<true>);
     } else {
-      GSB_LAUNCH_RENDER_T(kTilePixels / 2, render_compact_kernel<false, 2>);
+      GSB_LAUNCH_RENDER(render_table_kernel<false>);
     }
-#undef GSB_LAUNCH_RENDER_T
+#undef GSB_LAUNCH_RENDER
   }
   count_launch();
   return check_launch("render_kernel", stream, f.dbg);
@@ -1984,14 +1954,8 @@ int gsb_raster_forward_pair(const GsbRasterArgs* left, const GsbRasterArgs* righ
   const int pre_blocks = (left->P + kPreThreads - 1) / kPreThreads;
   {
     StageTimer tm(kStPreprocess, sl);
-    static const int occ = [] {  // A/B switch: GSB_PRE_OCC=4 -> 114 registers, no spills, 4 CTAs per SM
-      const char* e = getenv("GSB_PRE_OCC");
-      return e ? atoi(e) : 5;  // measured on C1: 0.194 ms (5 CTAs / SM, 96 registers, 48 B of spills) vs 0.209 ms (4 CTAs, 114)
-    }();
-    if (occ == 5)
-      preprocess_kernel<2, 5><<<pre_blocks, kPreThreads, 0, sl>>>(pp);
-    else
-      preprocess_kernel<2, 4><<<pre_blocks, kPreThreads, 0, sl>>>(pp);
+    // 5 CTAs per SM: measured on C1 at 0.194 ms (96 registers, 48 B of spills) vs 0.209 ms at 4 (114 registers, no spills)
+    preprocess_kernel<2, 5><<<pre_blocks, kPreThreads, 0, sl>>>(pp);
   }
   count_launch();
   if ((rc = check_launch("preprocess_kernel<2>", sl, fl.dbg))) return rc;

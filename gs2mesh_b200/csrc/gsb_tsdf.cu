@@ -271,14 +271,14 @@ constexpr int kSweep = 2;                                    // passes handled t
 //   (C) loads of the UPDATED pairs only: (tsdf, weight), colour, rgb -- all in flight together
 //   (D) fuse + store
 // ~60% of the voxels of a touched brick lie outside the truncation band and are never read or written.
-template <int kMinBlocks>
-__global__ void __launch_bounds__(kIntThreads, kMinBlocks) integrate_kernel(const FrameParams f, const float* __restrict__ depth,
-                                                                  const uint8_t* __restrict__ rgb, float4* __restrict__ tw,
-                                                                  float4* __restrict__ color,
-                                                                  const uint32_t* __restrict__ list,
-                                                                  uint32_t* __restrict__ counters,
-                                                                  const unsigned long long* __restrict__ hash_keys,
-                                                                  const uint32_t* __restrict__ hash_vals, uint32_t pool) {
+// Compiled for 4 CTAs per SM: 64 registers and a few spilled bytes at sm_90a, where 3 CTAs would give 80 and no spills.
+__global__ void __launch_bounds__(kIntThreads, 4) integrate_kernel(const FrameParams f, const float* __restrict__ depth,
+                                                                   const uint8_t* __restrict__ rgb, float4* __restrict__ tw,
+                                                                   float4* __restrict__ color,
+                                                                   const uint32_t* __restrict__ list,
+                                                                   uint32_t* __restrict__ counters,
+                                                                   const unsigned long long* __restrict__ hash_keys,
+                                                                   const uint32_t* __restrict__ hash_vals, uint32_t pool) {
   // a frame cannot queue more entries than the list holds (one per pool slot + the few a full pool refused)
   const uint32_t n = counters[kCntQueued];
   const int t = threadIdx.x;
@@ -760,18 +760,9 @@ int gsb_tsdf_integrate(GsbVolume* vol, const float* depth, const uint8_t* rgb, i
   const unsigned long long* hkeys = reinterpret_cast<const unsigned long long*>(d.hash_keys);
   {
     StageTimer tm(kStIntegrate, stream);
-    static const int occ = [] {  // A/B switch for profiling: GSB_INTEGRATE_OCC=3 -> 85 registers, no spills
-      const char* e = getenv("GSB_INTEGRATE_OCC");
-      return e ? atoi(e) : 4;
-    }();
-    if (occ == 3)
-      integrate_kernel<3><<<grid, kIntThreads, 0, stream>>>(f, depth, rgb, reinterpret_cast<float4*>(d.tsdf_weight),
-                                                            reinterpret_cast<float4*>(d.color), d.brick_list, d.counters, hkeys,
-                                                            d.hash_vals, d.pool_bricks);
-    else
-      integrate_kernel<4><<<grid, kIntThreads, 0, stream>>>(f, depth, rgb, reinterpret_cast<float4*>(d.tsdf_weight),
-                                                            reinterpret_cast<float4*>(d.color), d.brick_list, d.counters, hkeys,
-                                                            d.hash_vals, d.pool_bricks);
+    integrate_kernel<<<grid, kIntThreads, 0, stream>>>(f, depth, rgb, reinterpret_cast<float4*>(d.tsdf_weight),
+                                                       reinterpret_cast<float4*>(d.color), d.brick_list, d.counters, hkeys,
+                                                       d.hash_vals, d.pool_bricks);
   }
   count_launch();
   return check_launch("integrate_kernel", stream, false);

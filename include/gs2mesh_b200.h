@@ -65,32 +65,23 @@ int gsb_profile_collect(double* total_ms, uint64_t* samples, int n_stages);
  * Rasterizer
  * ------------------------------------------------------------------------------------------ */
 
-/* flags for GsbRasterArgs.flags */
+/* flags for GsbRasterArgs.flags; a call with any other bit set fails with GSB_ERR_INVALID */
 #define GSB_RASTER_EXACT_TILE_CULL 1u /* drop (Gaussian,tile) pairs that provably contribute to no
                                          pixel of the tile; image is bit-identical, num_rendered
                                          shrinks.  Off = reference rectangle binning
                                          (rasterizer_impl.cu:88-107).                          */
-#define GSB_RASTER_NO_TMA 2u          /* stage parameters with plain loads (debug / A-B only)  */
+#define GSB_RASTER_NO_TMA 2u          /* stage parameters with plain loads, the path unaligned inputs
+                                         always take (for tests: same results as bulk TMA)      */
 #define GSB_RASTER_DEBUG_SYNC 4u      /* synchronise + check after every stage, like debug=True
                                          (auxiliary.h:166-173)                                 */
 #define GSB_RASTER_CUB_SORT 8u        /* validation only: the reference's pipeline shape (P-sized scan,
                                          cub::DeviceRadixSort on tile|depth keys, host read of the
                                          instance count) instead of the in-library depth-presort +
                                          stable tile split                                      */
-#define GSB_RASTER_FAST_EXP 32u       /* blend with ex2.approx(power*log2e) instead of full-precision
-                                         expf: ~2e-7 relative on alpha (parity budget is 1e-4)   */
-/* A/B overrides of the library defaults, for tests and profiling (0 in a field = library default, which the
- * environment variables GSB_RENDER_IMPL / GSB_PRE_SH may also change):
- *   bits 8..10  blend kernel: 4 dual (per-warp compacted hit lists, 8x8 pixels per warp, the reference's exponent
- *               expression), 5 table (dual with per-column / per-row exponent tables, packed f32x2 and predicated
- *               accumulation; default, needs GSB_RASTER_FAST_EXP -- without it the dual kernel runs); 1..3 (variants
- *               removed in round 2) select dual
- *   bits 12..13 SH staging of full-degree blocks: 1 scalar reads, 2 16-byte reads (default), 3 per-lane bulk copies
- *               into padded slots + 16-byte reads
- * dual produces the reference's transmittance bit for bit when GSB_RASTER_FAST_EXP is off; table rounds the exponent
- * differently (~1e-6 relative on alpha). */
-#define GSB_RASTER_RENDER_IMPL(n) (((uint32_t)(n) & 7u) << 8)
-#define GSB_RASTER_SH_MODE(n) (((uint32_t)(n) & 3u) << 12)
+#define GSB_RASTER_FAST_EXP 32u       /* blend with ex2.approx in per-column / per-row exponent tables
+                                         (~1e-6 relative on alpha; parity budget is 1e-4).  Off =
+                                         the reference's exponent expression with full-precision
+                                         expf: transmittance bit for bit the reference's        */
 #define GSB_RASTER_PAIR_SHARED_DEPTH 64u /* gsb_raster_forward_pair only (left->flags): the caller asserts that both eyes see
                                          every Gaussian at the same view depth, i.e. viewmatrix[2], [6], [10], [14] are
                                          bitwise equal in the two argument blocks; ONE depth sort then serves both eyes.

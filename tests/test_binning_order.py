@@ -55,7 +55,8 @@ def test_depth_presort_plus_stable_tile_split_equals_reference_order():
 
 
 def test_digit_widths_do_not_change_a_stable_lsd_sort():
-    """8+5-bit and 7+6-bit digits (GSB_RADIX_SPLIT) sort 13-bit tile ids identically; 4 x 8 bits sort 32-bit depth keys."""
+    """8+5-bit and 7+6-bit digits (the radix sort's even split) sort 13-bit tile ids identically; 4 x 8 bits sort 32-bit
+    depth keys."""
     rng = np.random.default_rng(4)
     tile = rng.integers(0, 7500, size=20000).astype(np.uint64)
     vals = np.arange(20000)

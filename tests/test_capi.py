@@ -56,6 +56,33 @@ def test_argument_validation_without_gpu(gsb_lib):
     gsb_lib.gsb_tsdf_destroy(h)
 
 
+def test_undefined_flag_bits_are_refused(gsb_lib):
+    """A flags word with a bit outside the GSB_RASTER_* set fails validation, before anything is enqueued.  The blend-kernel
+    (bits 8..10) and SH-staging (bits 12..13) selector fields no longer exist; a caller still passing them gets an error."""
+    import ctypes as C
+
+    P, W, H, cap = 1000, 64, 48, 4000
+    need = gsb_lib.gsb_raster_workspace_bytes(P, W, H, cap)
+    ok = _lib.RASTER_EXACT_TILE_CULL | _lib.RASTER_FAST_EXP
+
+    def args(flags, workspace):
+        # any non-NULL pointers: validation only checks them for NULL, nothing is dereferenced before it passes
+        ptrs = {f: 256 for f in ("background", "means3D", "shs", "opacities", "scales", "rotations", "viewmatrix", "projmatrix",
+                                 "cam_pos", "out_color")}
+        return _lib.GsbRasterArgs(P=P, sh_degree=3, sh_coeffs=16, width=W, height=H, scale_modifier=1.0, tan_fovx=0.5,
+                                  tan_fovy=0.4, flags=flags, workspace=workspace, workspace_bytes=need, max_instances=cap, **ptrs)
+
+    for bit in (1 << 8, 1 << 9, 1 << 10, 1 << 12, 1 << 13, 1 << 31):
+        msg = b"undefined bits 0x%x" % bit
+        bad = args(ok | bit, 4096)
+        assert gsb_lib.gsb_raster_forward(C.byref(bad), None) == _lib.GSB_ERR_INVALID
+        assert msg in gsb_lib.gsb_last_error()
+        good = args(ok, 8192)
+        for left, right in ((bad, good), (good, bad)):
+            assert gsb_lib.gsb_raster_forward_pair(C.byref(left), C.byref(right), None, None) == _lib.GSB_ERR_INVALID
+            assert msg in gsb_lib.gsb_last_error()
+
+
 def test_struct_layout_matches_header():
     import ctypes as C
 

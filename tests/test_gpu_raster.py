@@ -255,17 +255,22 @@ def test_undersized_workspace_async_flags_frame_and_stays_in_bounds(gsb_lib, cud
 
 
 def test_fast_exp_stays_inside_parity_budget(oracle, gsb_lib, cuda_device):
-    """GSB_RASTER_FAST_EXP (ex2.approx in the blend loop, the Renderer's default) vs the reference
-    rasterizer / oracle: still within 1e-4 relative with the same outlier budget."""
+    """GSB_RASTER_FAST_EXP (the table kernel: ex2.approx of a log2-domain exponent, the Renderer's default) vs the
+    full-precision expf kernel and the reference rasterizer / oracle: same instance lists, still within 1e-4 relative with
+    the same outlier budget."""
     from gs2mesh_b200 import _lib
 
-    for n, W, H, seed in [(10000, 640, 480, 1), (3000, 320, 240, 0)]:
+    # 333x250: ragged tiles on both axes (no golden reference data at that size)
+    for n, W, H, seed in [(10000, 640, 480, 1), (3000, 320, 240, 0), (3000, 333, 250, 5)]:
         g, vt = _case(n, W, H, seed)
         inp = _np_inputs(g, vt)
         fast = _ours(cuda_device, inp, flags=_lib.RASTER_EXACT_TILE_CULL | _lib.RASTER_FAST_EXP)
         exact = _ours(cuda_device, inp, flags=_lib.RASTER_EXACT_TILE_CULL)
+        np.testing.assert_array_equal(fast["counts"], exact["counts"])
         r = compare_images(fast["color"], exact["color"])
         assert r["frac_bad"] <= BUDGET and r["median"] <= 1e-6, r
+        if (n, W, H, seed) not in REF_CASES:
+            continue
         ref = _golden_ref(n, W, H, seed)
         _assert_parity(_at(fast["color"], ref["pixels"]), ref["color"], "fast-exp color vs reference")
         _assert_parity(_at(fast["final_T"], ref["pixels"]), ref["final_T"], "fast-exp final_T vs reference")
@@ -273,52 +278,9 @@ def test_fast_exp_stays_inside_parity_budget(oracle, gsb_lib, cuda_device):
         _assert_parity(fast["depth"], o["depth"], "fast-exp depth vs oracle")
 
 
-@pytest.mark.parametrize("fast", [False, True])
-def test_blend_kernel_variants_agree(gsb_lib, cuda_device, fast):
-    """dual (the reference's exponent expression) vs table (default: log2-domain exponent from per-column / per-row terms, packed
-    pixel pairs per lane, predicated accumulation): same thresholds of forward.cu:336-353, same instance lists; alpha differs by rounding
-    (~1e-6 relative), so the images agree like against the reference.  Without GSB_RASTER_FAST_EXP both names run the dual
-    kernel with full-precision expf: bit-identical."""
-    from gs2mesh_b200 import _lib
-
-    for n, W, H, seed in [(10000, 640, 480, 1), (3000, 333, 250, 5)]:  # 333x250: ragged tiles on both axes
-        g, vt = _case(n, W, H, seed)
-        inp = _np_inputs(g, vt)
-        base = _lib.RASTER_EXACT_TILE_CULL | (_lib.RASTER_FAST_EXP if fast else 0)
-        outs = {name: _ours(cuda_device, inp, flags=base | _lib.RASTER_RENDER_IMPL(name)) for name in _lib.RENDER_IMPLS}
-        ref, out = outs["dual"], outs["table"]
-        np.testing.assert_array_equal(out["counts"], ref["counts"])
-        if fast:
-            for k in ("color", "final_T", "depth"):
-                cmp = compare_images(out[k], ref[k])
-                assert cmp["frac_bad"] <= BUDGET and cmp["median"] <= 2e-6, (k, cmp)
-            assert np.abs(out["color"] - ref["color"]).max() > 0  # they are different kernels
-        else:
-            for k in ("color", "final_T", "depth"):
-                np.testing.assert_array_equal(out[k], ref[k], err_msg=k)
-        legacy = _ours(cuda_device, inp, flags=base | _lib.RASTER_RENDER_IMPL(2))  # a removed variant's number selects dual
-        np.testing.assert_array_equal(legacy["color"], ref["color"])
-
-
-def test_sh_staging_variants_agree(gsb_lib, cuda_device):
-    """scalar / 16-byte / padded-slot staging of the SH block (also without TMA and on the ragged last warp).  The two
-    register-fed variants run the same instructions and are bit-identical; the scalar variant evaluates the same
-    expression from shared-memory operands, where ptxas fuses one multiply-add differently: colours within 2 ulp,
-    everything that decides binning and blending order identical."""
-    from gs2mesh_b200 import _lib
-
-    g, vt = _case(4099, 320, 240, seed=22)
-    inp = _np_inputs(g, vt)
-    for extra in (0, _lib.RASTER_NO_TMA):
-        outs = {m: _ours(cuda_device, inp, flags=_lib.RASTER_EXACT_TILE_CULL | extra | _lib.RASTER_SH_MODE(m)) for m in _lib.SH_MODES}
-        for k in ("color", "depth", "final_T", "radii", "counts"):
-            np.testing.assert_array_equal(outs["padded"][k], outs["vec"][k], err_msg=k)
-        for k in ("depth", "final_T", "radii", "counts"):
-            np.testing.assert_array_equal(outs["scalar"][k], outs["vec"][k], err_msg=k)
-        np.testing.assert_allclose(outs["scalar"]["color"], outs["vec"]["color"], rtol=3e-7, atol=3e-7)
-
-
 def test_tma_staging_equals_plain_loads(gsb_lib, cuda_device):
+    """Bulk-TMA staging (full warps) vs plain loads (GSB_RASTER_NO_TMA; always on the ragged last warp), both feeding the
+    16-byte shared-memory reads of the full-degree SH block."""
     from gs2mesh_b200 import _lib
 
     g, vt = _case(4099, 320, 240, seed=21)  # 4099 = 128*32 + 3: exercises the ragged last warp
