@@ -141,18 +141,38 @@ __global__ void __launch_bounds__(256) grid_scatter_kernel(const GsbPointGrid g,
   g.ids[g.cell_start[c] + atomicAdd(&fill[c], 1u)] = i;
 }
 
-// Rings of cells at Chebyshev distance k around the query's (unclamped) cell.  Every point in a ring > k lies at least
-// k*h away, so the search stops once the best distance is below that bound (with a relative margin far above the
-// rounding error of the distance expression), or once k*h reaches max_dist.  Returns the nearest point (lowest index
-// among equal squared distances; -1 if none) and its ((dx*dx)+dy*dy)+dz*dz; a point at max_dist or beyond may be missed.
+// Rings of cells at Chebyshev distance k around the query's cell.  Every point in a ring > k lies at least k*h away, so
+// the search stops once the best distance is below that bound, or once k*h reaches max_dist.  Returns the nearest point
+// (lowest index among equal squared distances; -1 if none) and its ((dx*dx)+dy*dy)+dz*dz; a point at max_dist or beyond
+// may be missed.  A query with a coordinate that is not finite returns (+inf, -1) without searching.
+//
+// The query's cell is clamped, in double, to [-kFarCells, dims-1 + kFarCells] per axis: a query farther out gets a cell
+// nearer the grid, which only shrinks the ring bounds (k-1)*h, so they stay lower bounds; k and qc +- k stay far from
+// int64 overflow, and the rings walked stay within kFarCells + dims.
+//
+// The ring bound's relative margin kRingMargin must exceed the rounding error of the cell indices.  A query's or a
+// point's index (p - o) / h rounds twice, so it is off by at most 2^-52 * |index| cells.  A point in ring k of a query
+// has |index| < dims and the query |index| <= k + dims, so the two are off by at most 2^-52 * (k + 2*dims) cells, which
+// stays below kRingMargin * (k - 1) for every k >= 2 while dims <= kMaxAxisCells (9.3e-10 at k = 2; grid_ok refuses
+// larger axes).  The distance expression's own rounding (a few ulp) is far below the margin.  PointGrid's cell floor of
+// (hi - lo) / 1e6 keeps every axis at about 1e6 cells: a change to that floor must keep it within kMaxAxisCells.
+constexpr double kFarCells = 1099511627776.0;  // 2^40
+constexpr double kRingMargin = 1e-9;
+constexpr int kMaxAxisCells = 1 << 21;
+
 struct Nearest {
   double d2;
   long long id;
 };
 
+__device__ __forceinline__ long long query_cell(double p, double o, double h, int dim) {
+  return (long long)fmin(fmax(floor((p - o) / h), -kFarCells), (double)(dim - 1) + kFarCells);
+}
+
 __device__ __forceinline__ Nearest ring_nearest(const GsbPointGrid& g, double qx, double qy, double qz, double max_dist) {
-  const long long qc[3] = {(long long)floor((qx - g.origin[0]) / g.cell), (long long)floor((qy - g.origin[1]) / g.cell),
-                           (long long)floor((qz - g.origin[2]) / g.cell)};
+  if (!(isfinite(qx) && isfinite(qy) && isfinite(qz))) return {INFINITY, -1};
+  const long long qc[3] = {query_cell(qx, g.origin[0], g.cell, g.dims[0]), query_cell(qy, g.origin[1], g.cell, g.dims[1]),
+                           query_cell(qz, g.origin[2], g.cell, g.dims[2])};
   // first ring that can reach the grid, last ring that still meets it
   long long k0 = 0, k1 = 0;
 #pragma unroll
@@ -163,7 +183,7 @@ __device__ __forceinline__ Nearest ring_nearest(const GsbPointGrid& g, double qx
   }
   double best2 = INFINITY;
   long long best = -1;
-  const double margin = 1.0 - 1e-9;
+  const double margin = 1.0 - kRingMargin;
   for (long long k = k0; k <= k1; ++k) {
     const double lb = (double)(k > 0 ? k - 1 : 0) * g.cell * margin;  // every point of ring k is at least this far away
     if (lb >= max_dist) break;
@@ -274,7 +294,7 @@ bool grid_ok(const GsbPointGrid* g) {
   if (!g || g->n_points < 0 || (g->n_points && !g->points) || !g->cell_start || !(g->cell > 0.0)) return false;
   double cells = 1.0;
   for (int a = 0; a < 3; ++a) {
-    if (g->dims[a] <= 0) return false;
+    if (g->dims[a] <= 0 || g->dims[a] > kMaxAxisCells) return false;  // the ring bound's margin covers kMaxAxisCells
     cells *= g->dims[a];
   }
   return cells < 2147483647.0;

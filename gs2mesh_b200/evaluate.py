@@ -63,12 +63,33 @@ def sample_mesh_points(vertices, triangles, density=0.2):
     return out
 
 
+def grid_layout(lo, hi, core, n, cells_per_point=4.0, min_cell=0.0, max_cells=1 << 26):
+    """(cell, dims) of PointGrid for n points with bounds lo / hi and 1%..99% quantile extent `core` per axis.
+
+    The cell never falls below (hi - lo).max() * 1e-6, so no axis has more than about 1e6 cells: the ring search's
+    rounding margin (gsb_eval.cu, kRingMargin) covers up to 2^21.  When the points coincide (an extent of 1e-294 or less)
+    the cell is tied to the coordinates' magnitude instead, max(|lo|, |hi|, 1) * 2^-30: one cell holds them all, and the
+    cell stays a normal number, so the search's distance bounds keep their precision."""
+    lo, hi, core = (np.asarray(x, dtype=np.float64) for x in (lo, hi, core))
+    big = float(core.max())
+    cell = (float(np.prod(np.maximum(core, big * 1e-3))) / (cells_per_point * n)) ** (1.0 / 3.0) if big > 0 else 0.0
+    cell = max(cell, float(min_cell), float((hi - lo).max()) * 1e-6)
+    if not cell > 1e-300:
+        cell = max(float(np.abs(lo).max()), float(np.abs(hi).max()), 1.0) * 2.0 ** -30
+    ext = hi - lo
+    while True:
+        dims = [int(e // cell) + 1 for e in ext]
+        if dims[0] * dims[1] * dims[2] <= max_cells:
+            return cell, dims
+        cell *= 1.25
+
+
 class PointGrid:
     """Reference points bucketed into a uniform grid (gsb_eval_grid_build), reusable for many nearest() queries.
 
     The cell size comes from the point spacing inside the 1%..99% quantile box of each axis (so a few far floaters do not
     stretch the cells over the whole object), never below min_cell; the grid then covers every point, and the cell grows
-    only when that would need more than max_cells cells."""
+    only when that would need more than max_cells cells (grid_layout)."""
 
     def __init__(self, reference, cells_per_point=4.0, min_cell=0.0, max_cells=1 << 26):
         self.points = _points(reference)
@@ -84,15 +105,7 @@ class PointGrid:
         srt = sub.sort(dim=0).values
         m = srt.shape[0]
         core = (srt[min(m - 1, int(0.99 * m))] - srt[int(0.01 * m)]).cpu().numpy()
-        big = float(core.max())
-        cell = (float(np.prod(np.maximum(core, big * 1e-3))) / (cells_per_point * n)) ** (1.0 / 3.0) if big > 0 else 0.0
-        cell = max(cell, float(min_cell), float((hi - lo).max()) * 1e-6, 1e-300)
-        ext = hi - lo
-        while True:
-            dims = [int(e // cell) + 1 for e in ext]
-            if dims[0] * dims[1] * dims[2] <= max_cells:
-                break
-            cell *= 1.25
+        cell, dims = grid_layout(lo, hi, core, n, cells_per_point, min_cell, max_cells)
         self.origin, self.cell, self.dims = lo, cell, dims
         cells = dims[0] * dims[1] * dims[2]
         self.cell_start = torch.empty(cells + 1, dtype=torch.int64, device=dev)
@@ -119,7 +132,7 @@ class PointGrid:
 def nearest(queries, reference, max_dist=math.inf):
     """Exact 1-NN of every query among `reference` -> (dist fp64 [N], idx int64 [N]) on the device.  dist equals sklearn's
     kd_tree kneighbors distance sqrt(((dx*dx)+dy*dy)+dz*dz) bit for bit; among equal squared distances the lowest index
-    wins.  Queries with nothing closer than max_dist get (+inf, -1)."""
+    wins.  Queries with nothing closer than max_dist, and queries with a NaN or infinite coordinate, get (+inf, -1)."""
     return PointGrid(reference).nearest(queries, max_dist)
 
 
@@ -150,7 +163,7 @@ def radius_downsample(points, radius, seed=0, order=None):
     n = p.shape[0]
     if order is None:
         order = np.random.default_rng(seed).permutation(n)
-    order = torch.as_tensor(np.asarray(order, dtype=np.int64)).to(dev)
+    order = torch.as_tensor(np.ascontiguousarray(order, dtype=np.int64)).to(dev)  # a reversed view has negative strides
     if order.shape != (n,):
         raise ValueError("radius_downsample: order must be a permutation of the points")
     shuffled = p[order].contiguous()

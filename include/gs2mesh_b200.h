@@ -344,7 +344,7 @@ int gsb_eval_sample_emit(const double* vertices, int64_t n_vertices, const int64
 typedef struct GsbPointGrid {
   double origin[3];
   double cell;              /* cell edge length, > 0                                   */
-  int32_t dims[3];          /* cells per axis; dims[0]*dims[1]*dims[2] < 2^31           */
+  int32_t dims[3];          /* cells per axis, each <= 2^21; dims[0]*dims[1]*dims[2] < 2^31 */
   const double* points;     /* device double [n_points,3]                             */
   int64_t n_points;
   int64_t* cell_start;      /* device int64 [cells+1]: ids of cell c are ids[cell_start[c] .. cell_start[c+1]) */
@@ -357,7 +357,8 @@ int gsb_eval_grid_build(const GsbPointGrid* grid, void* workspace, size_t worksp
 /* Exact 1-nearest neighbour of every query among the grid's points: dist = sqrt(((dx*dx)+dy*dy)+dz*dz) (sklearn's kd_tree
  * kneighbors distance, bit for bit), index = the nearest point (lowest index among equal squared distances).  Queries
  * with no point closer than max_dist get dist = +inf, index = -1, and the search stops there; max_dist = +inf searches
- * until the nearest point is found. */
+ * until the nearest point is found.  A query with a NaN or infinite coordinate gets dist = +inf, index = -1 without a
+ * search.  Grids with more than 2^21 cells on an axis are refused (GSB_ERR_INVALID) by every gsb_eval_* grid call. */
 int gsb_eval_nearest(const GsbPointGrid* grid, const double* queries, int64_t n_queries, double max_dist, double* dist,
                      int64_t* index, void* stream);
 /* Greedy radius downsampling of the grid's points in index order (eval.py:88-93): keep[p] = 1 iff no earlier kept point q
@@ -385,7 +386,8 @@ int gsb_eval_radius_downsample(const GsbPointGrid* grid, double radius, uint8_t*
  *                              voxel_size * INT_MAX < the padded extent (Open3D's "voxel_size is too small") or when the
  *                              voxel keys need more than 63 bits.  n_points < 2^31.
  *   gsb_eval_icp_correspond    index[i] = the nearest grid point with ((dx*dx)+dy*dy)+dz*dz < radius*radius, else -1;
- *                              dist2[i] its squared distance (+inf for -1).
+ *                              dist2[i] its squared distance (+inf for -1).  A source point with a NaN or infinite
+ *                              coordinate gets -1.
  *   gsb_eval_icp_moments       sums over the correspondences (index[i] >= 0) with a fixed reduction tree (the same bits on
  *                              every run): pass 0 writes out[0..6] = (sum dist2, sum source xyz, sum target[index] xyz);
  *                              pass 1, given means = host double [6] (source mean, target mean), writes out[0..8] =

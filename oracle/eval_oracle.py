@@ -66,6 +66,29 @@ def nearest(queries, reference):
     return distance(queries, reference[idx]), idx
 
 
+def nearest_exact(queries, reference, max_dist=np.inf, chunk=1 << 22):
+    """(dist, idx) of gsb_eval_nearest by brute force in fp64: the minimum of ((dx*dx)+dy*dy)+dz*dz over every reference
+    point, the lowest index among equal minima, dist = its sqrt.  Queries whose dist is not below max_dist, and queries
+    with a coordinate that is not finite, get (+inf, -1).  Works on blocks of about `chunk` query-point pairs."""
+    q = np.asarray(queries, dtype=np.float64).reshape(-1, 3)
+    ref = np.asarray(reference, dtype=np.float64).reshape(-1, 3)
+    dist = np.full(len(q), np.inf)
+    idx = np.full(len(q), -1, dtype=np.int64)
+    if len(ref) == 0:
+        return dist, idx
+    step = max(1, chunk // len(ref))
+    for a in range(0, len(q), step):
+        with np.errstate(over="ignore", invalid="ignore"):  # far or non-finite queries: inf / nan, handled below
+            d = q[a:a + step, None, :] - ref[None, :, :]
+            dd = (d[..., 0] * d[..., 0] + d[..., 1] * d[..., 1]) + d[..., 2] * d[..., 2]
+        k = dd.argmin(axis=1)  # the first minimum: the lowest index
+        best = np.sqrt(dd[np.arange(len(k)), k])
+        hit = (best < max_dist) & np.isfinite(q[a:a + step]).all(axis=1)
+        dist[a:a + step] = np.where(hit, best, np.inf)
+        idx[a:a + step] = np.where(hit, k, -1)
+    return dist, idx
+
+
 def radius_downsample(points, thresh):
     """Keep mask of eval.py:88-93 for points already in shuffled order: the literal sequential loop over radius neighbours,
     a neighbour being a point with ((dx*dx)+dy*dy)+dz*dz <= thresh*thresh (sklearn's radius test on reduced distances)."""
