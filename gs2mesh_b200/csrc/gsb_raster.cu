@@ -170,17 +170,18 @@ __device__ __forceinline__ bool rect_can_contribute(float gxp, float gyp, const 
   const float qh = f.a * ex * ex + 2.f * f.b * ex * ey + f.c * ey * ey;
   return fminf(qv, qh) <= f.two_tau + margin;
 }
+// A non-degenerate footprint and its centre as two float4 (x, y, a, b), (c, nb_a, nb_c, two_tau), as lanes share it.
+__device__ __forceinline__ void publish_footprint(float4* slot, float px, float py, const Footprint& f) {
+  slot[0] = make_float4(px, py, f.a, f.b);
+  slot[1] = make_float4(f.c, f.nb_a, f.nb_c, f.two_tau);
+}
+__device__ __forceinline__ Footprint read_footprint(const float4& q0, const float4& q1) {
+  return Footprint{q0.z, q0.w, q1.x, q1.y, q1.z, q1.w, false};
+}
 // __noinline__: the counting and the emitting kernel must execute the same instructions.
 __device__ __noinline__ bool tile_can_contribute(float gxp, float gyp, float a, float b, float c, float nb_a, float nb_c,
                                                  float two_tau, uint32_t tx, uint32_t ty) {
-  Footprint f;
-  f.a = a;
-  f.b = b;
-  f.c = c;
-  f.nb_a = nb_a;
-  f.nb_c = nb_c;
-  f.two_tau = two_tau;
-  f.degenerate = false;
+  const Footprint f = read_footprint(make_float4(gxp, gyp, a, b), make_float4(c, nb_a, nb_c, two_tau));
   const float x0 = (float)(tx * kTile), y0 = (float)(ty * kTile);
   return rect_can_contribute(gxp, gyp, f, x0, y0, x0 + (kTile - 1), y0 + (kTile - 1));
 }
@@ -190,7 +191,6 @@ __device__ __noinline__ bool tile_can_contribute(float gxp, float gyp, float a, 
 // rounding allowance as rect_can_contribute's margin (its S term is <= 4 tau k over the box, k = ac/det); very elongated
 // conics (k > 1000) keep the reference rectangle.  Explicitly rounded operations only: the binning, the emitting and the
 // validation kernel must all arrive at the same rectangle.
-constexpr uint32_t kRectLarge = 0xffffffffu;  // packed-rectangle sentinel: no mask stored, re-test when emitting
 __device__ __forceinline__ TileRect shrink_rect(TileRect r, float px, float py, const Footprint& f) {
   if (f.degenerate) return r;
   const float ac = __fmul_rn(f.a, f.c);
@@ -223,6 +223,111 @@ __device__ __forceinline__ TileRect shrink_rect(TileRect r, float px, float py, 
   return r;
 }
 
+// A Gaussian's candidate tiles: the reference rectangle, under exact culling shrunk to the ellipse's (shrink_rect), and
+// whether each of its tiles must be tested.  The binning, the emitting and the validation kernel all decide here.
+struct Candidate {
+  TileRect rc;
+  Footprint fp;  // make_footprint(1, 0, 1, 0) without exact culling
+  bool test;     // exact culling of a positive-definite conic: tiles are tested, not all kept
+  uint32_t w, area;
+};
+__device__ __forceinline__ Candidate no_candidate() {  // a Gaussian binned nowhere
+  return Candidate{TileRect{0, 0, 0, 0}, make_footprint(1.f, 0.f, 1.f, 0.f), false, 0u, 0u};
+}
+// conic = (a, b, c, ·) as in recB; taken by reference so that the emit kernels only load it under exact culling
+__device__ __forceinline__ Candidate make_candidate(float px, float py, int radius, const float4& conic, float opacity,
+                                                    uint32_t gx, uint32_t gy, bool exact) {
+  Candidate cd = no_candidate();
+  cd.rc = tile_rect(px, py, radius, gx, gy);
+  if (exact) {
+    cd.fp = make_footprint(conic.x, conic.y, conic.z, 2.f * logf(255.f * opacity));
+    cd.test = !cd.fp.degenerate;
+    cd.rc = shrink_rect(cd.rc, px, py, cd.fp);
+  }
+  cd.w = cd.rc.x1 - cd.rc.x0;
+  cd.area = cd.w * (cd.rc.y1 - cd.rc.y0);
+  return cd;
+}
+
+// A candidate rectangle of at most kMaskTiles tiles packed into the word the emit pass replays its mask with:
+// x0 | y0 << kRectCoordBits | (w - 1) << 2 kRectCoordBits.  kRectLarge: no mask stored, re-test when emitting.
+constexpr uint32_t kMaskTiles = 64;
+constexpr uint32_t kRectCoordBits = 13, kRectWidthBits = 6;
+constexpr uint32_t kRectCoordMax = (1u << kRectCoordBits) - 1u;
+constexpr uint32_t kRectLarge = 0xffffffffu;
+static_assert(2 * kRectCoordBits + kRectWidthBits == 32, "the packed rectangle is one word");
+static_assert(kMaskTiles == 1u << kRectWidthBits, "w - 1 of a rectangle of up to kMaskTiles tiles fills the width field");
+__device__ __forceinline__ uint32_t pack_rect(uint32_t x0, uint32_t y0, uint32_t w) {
+  return x0 | (y0 << kRectCoordBits) | ((w - 1u) << (2 * kRectCoordBits));
+}
+__device__ __forceinline__ uint3 unpack_rect(uint32_t word) {  // (x0, y0, w)
+  return make_uint3(word & kRectCoordMax, (word >> kRectCoordBits) & kRectCoordMax, (word >> (2 * kRectCoordBits)) + 1u);
+}
+
+// Slot k of a rectangle w tiles wide, row-major -> (column, row).  For k < 64, w <= 64, (k + 0.5) / w is never within
+// rounding distance of an integer, so the approximate division floors to the exact row.
+__device__ __forceinline__ uint2 rect_slot(uint32_t k, uint32_t w) {
+  const uint32_t row = (uint32_t)__float2int_rd(__fdividef((float)k + 0.5f, (float)w));
+  return make_uint2(k - row * w, row);
+}
+
+// Warp-flattened slots: each lane's `cand` slots laid end to end in lane order.  warp_inclusive_sum gives a lane the end
+// of its slots; slot_owner the lane holding flattened slot fidx, the first whose inclusive sum exceeds fidx (for a valid
+// slot one of the 32 lanes: 5 halvings settle it).
+__device__ __forceinline__ uint32_t warp_inclusive_sum(uint32_t cand) {
+  const int lane = threadIdx.x & 31;
+  uint32_t incl = cand;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const uint32_t v = __shfl_up_sync(0xffffffffu, incl, o);
+    if (lane >= o) incl += v;
+  }
+  return incl;
+}
+__device__ __forceinline__ int slot_owner(uint32_t incl, uint32_t fidx) {
+  int lo = 0, hi = 31;
+#pragma unroll
+  for (int step = 0; step < 5; ++step) {
+    const int mid = (lo + hi) >> 1;
+    const uint32_t v = __shfl_sync(0xffffffffu, incl, mid);
+    if (v <= fidx)
+      lo = mid + 1;
+    else
+      hi = mid;
+  }
+  return lo;
+}
+
+// Rectangles too large for a mask: the whole warp tests the tiles of each lane with `large` set, in lane order, 32 per
+// step.  For each such lane it calls source(lane), which returns the callback run after every step:
+// step(tiles kept in earlier steps, keep, ballot, tx, ty).
+template <class Source>
+__device__ __forceinline__ void walk_large_rects(bool large, float px, float py, const Candidate& cd, Source source) {
+  const int lane = threadIdx.x & 31;
+  unsigned todo = __ballot_sync(0xffffffffu, large);
+  while (todo) {
+    const int src = __ffs(todo) - 1;
+    todo &= todo - 1;
+    const float spx = __shfl_sync(0xffffffffu, px, src), spy = __shfl_sync(0xffffffffu, py, src);
+    const float sa = __shfl_sync(0xffffffffu, cd.fp.a, src), sb = __shfl_sync(0xffffffffu, cd.fp.b, src);
+    const float sc = __shfl_sync(0xffffffffu, cd.fp.c, src), st = __shfl_sync(0xffffffffu, cd.fp.two_tau, src);
+    const float sna = __shfl_sync(0xffffffffu, cd.fp.nb_a, src), snc = __shfl_sync(0xffffffffu, cd.fp.nb_c, src);
+    const bool stest = __shfl_sync(0xffffffffu, (int)cd.test, src) != 0;
+    const uint32_t sx0 = __shfl_sync(0xffffffffu, cd.rc.x0, src), sy0 = __shfl_sync(0xffffffffu, cd.rc.y0, src);
+    const uint32_t sw = __shfl_sync(0xffffffffu, cd.w, src), sarea = __shfl_sync(0xffffffffu, cd.area, src);
+    auto step = source(src);
+    uint32_t done = 0;
+    for (uint32_t base = 0; base < sarea; base += 32) {
+      const uint32_t k = base + lane;
+      const uint32_t tx = sx0 + k % sw, ty = sy0 + k / sw;
+      const bool keep = k < sarea && (!stest || tile_can_contribute(spx, spy, sa, sb, sc, sna, snc, st, tx, ty));
+      const unsigned votes = __ballot_sync(0xffffffffu, keep);
+      step(done, keep, votes, tx, ty);
+      done += __popc(votes);
+    }
+  }
+}
+
 // Warp-flattened binning.  The candidate tiles of the warp's 32 Gaussians (rectangles of up to
 // kMaskTiles tiles) are laid end to end and tested 32 at a time with every lane busy, instead of
 // each lane looping over its own rectangle.  Returns this lane's kept-tile count; for rectangles
@@ -230,77 +335,35 @@ __device__ __forceinline__ TileRect shrink_rect(TileRect r, float px, float py, 
 // replay the decision without re-testing.  Larger rectangles are counted cooperatively (and
 // re-tested by the emit pass with the same __noinline__ routine, so both passes agree).
 // `stage` = 32 x 2 float4 of per-warp shared memory the lanes publish their footprint in.
-constexpr uint32_t kMaskTiles = 64;
 __device__ __forceinline__ uint32_t bin_gaussians_warp(bool active, float px, float py, float ca, float cb, float cc,
                                                        float opacity, int radius, uint32_t gx, uint32_t gy, bool exact,
                                                        float4* stage, uint64_t& mask, uint32_t& rect_word) {
   const int lane = threadIdx.x & 31;
-  TileRect rc{0, 0, 0, 0};
-  uint32_t w = 0, area = 0;
-  Footprint fp = make_footprint(1.f, 0.f, 1.f, 0.f);
-  bool test = false;
-  if (active) {
-    rc = tile_rect(px, py, radius, gx, gy);
-    if (exact) {
-      fp = make_footprint(ca, cb, cc, 2.f * logf(255.f * opacity));
-      test = !fp.degenerate;
-      rc = shrink_rect(rc, px, py, fp);
-    }
-    w = rc.x1 - rc.x0;
-    area = w * (rc.y1 - rc.y0);
-  }
+  Candidate cd = no_candidate();
+  if (active) cd = make_candidate(px, py, radius, make_float4(ca, cb, cc, 0.f), opacity, gx, gy, exact);
   mask = 0ull;
-  const bool small = active && area <= kMaskTiles;
-  // what the emit pass needs to replay the mask: x0 (13 bits) | y0 (13 bits) | w - 1 (6 bits)
-  rect_word = (small && area != 0) ? (rc.x0 | (rc.y0 << 13) | ((w - 1u) << 26)) : kRectLarge;
-  if (small && !test) mask = area == 64 ? ~0ull : ((1ull << area) - 1ull);  // rectangle binning: everything kept
-  const uint32_t cand = (small && test) ? area : 0u;
-  uint32_t incl = cand;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const uint32_t v = __shfl_up_sync(0xffffffffu, incl, o);
-    if (lane >= o) incl += v;
-  }
+  const bool small = active && cd.area <= kMaskTiles;
+  rect_word = (small && cd.area != 0) ? pack_rect(cd.rc.x0, cd.rc.y0, cd.w) : kRectLarge;
+  if (small && !cd.test) mask = cd.area == 64 ? ~0ull : ((1ull << cd.area) - 1ull);  // rectangle binning: everything kept
+  const uint32_t cand = (small && cd.test) ? cd.area : 0u;
+  const uint32_t incl = warp_inclusive_sum(cand);
   const uint32_t excl = incl - cand;
   const uint32_t total = __shfl_sync(0xffffffffu, incl, 31);
-  // publish what a tester needs to know about my Gaussian
-  stage[2 * lane] = make_float4(px, py, fp.a, fp.b);
-  stage[2 * lane + 1] = make_float4(fp.c, fp.nb_a, fp.nb_c, fp.two_tau);
-  const uint32_t pack0 = rc.x0 | (rc.y0 << 16);  // tile coordinates < 65536
-  const uint32_t pack1 = w | (excl << 8);          // w <= 64, excl <= 31 * 64
+  publish_footprint(stage + 2 * lane, px, py, cd.fp);
+  const uint32_t pack0 = cd.rc.x0 | (cd.rc.y0 << 16);  // tile coordinates < 65536
+  const uint32_t pack1 = cd.w | (excl << 8);             // w <= 64, excl <= 31 * 64
   __syncwarp();
   for (uint32_t w0 = 0; w0 < total; w0 += 32) {
     const uint32_t fidx = w0 + lane;
-    // owner = first lane whose inclusive prefix exceeds fidx
-    int lo = 0, hi = 31;  // the owner of a valid slot is one of the 32 lanes: 5 halvings settle it
-#pragma unroll
-    for (int step = 0; step < 5; ++step) {
-      const int mid = (lo + hi) >> 1;
-      const uint32_t v = __shfl_sync(0xffffffffu, incl, mid);
-      if (v <= fidx)
-        lo = mid + 1;
-      else
-        hi = mid;
-    }
-    const int owner = lo;
+    const int owner = slot_owner(incl, fidx);
     const uint32_t o0 = __shfl_sync(0xffffffffu, pack0, owner), o1 = __shfl_sync(0xffffffffu, pack1, owner);
     bool keep = false;
     if (fidx < total) {
       const float4 q0 = stage[2 * owner], q1 = stage[2 * owner + 1];
-      const uint32_t ow = o1 & 0xffu, k = fidx - (o1 >> 8);
-      // k / ow for k < 64, ow <= 64: (k + 0.5) / ow is never within rounding distance of an integer
-      const uint32_t row = (uint32_t)__float2int_rd(__fdividef((float)k + 0.5f, (float)ow));
-      const uint32_t tx = (o0 & 0xffffu) + (k - row * ow), ty = (o0 >> 16) + row;
-      Footprint f;
-      f.a = q0.z;
-      f.b = q0.w;
-      f.c = q1.x;
-      f.nb_a = q1.y;
-      f.nb_c = q1.z;
-      f.two_tau = q1.w;
-      f.degenerate = false;
+      const uint2 slot = rect_slot(fidx - (o1 >> 8), o1 & 0xffu);
+      const uint32_t tx = (o0 & 0xffffu) + slot.x, ty = (o0 >> 16) + slot.y;
       const float x0 = (float)(tx * kTile), y0 = (float)(ty * kTile);
-      keep = rect_can_contribute(q0.x, q0.y, f, x0, y0, x0 + (kTile - 1), y0 + (kTile - 1));
+      keep = rect_can_contribute(q0.x, q0.y, read_footprint(q0, q1), x0, y0, x0 + (kTile - 1), y0 + (kTile - 1));
     }
     const unsigned votes = __ballot_sync(0xffffffffu, keep);
     // collect the votes that belong to my own rectangle
@@ -312,27 +375,12 @@ __device__ __forceinline__ uint32_t bin_gaussians_warp(bool active, float px, fl
     }
   }
   uint32_t kept = small ? (uint32_t)__popcll(mask) : 0u;
-  // rectangles too large for a mask: whole warp per Gaussian, count only
-  unsigned todo = __ballot_sync(0xffffffffu, active && !small);
-  while (todo) {
-    const int src = __ffs(todo) - 1;
-    todo &= todo - 1;
-    const float spx = __shfl_sync(0xffffffffu, px, src), spy = __shfl_sync(0xffffffffu, py, src);
-    const float sa = __shfl_sync(0xffffffffu, fp.a, src), sb = __shfl_sync(0xffffffffu, fp.b, src);
-    const float sc = __shfl_sync(0xffffffffu, fp.c, src), st = __shfl_sync(0xffffffffu, fp.two_tau, src);
-    const float sna = __shfl_sync(0xffffffffu, fp.nb_a, src), snc = __shfl_sync(0xffffffffu, fp.nb_c, src);
-    const bool stest = __shfl_sync(0xffffffffu, (int)test, src) != 0;
-    const uint32_t sx0 = __shfl_sync(0xffffffffu, rc.x0, src), sy0 = __shfl_sync(0xffffffffu, rc.y0, src);
-    const uint32_t sw = __shfl_sync(0xffffffffu, w, src), sarea = __shfl_sync(0xffffffffu, area, src);
-    uint32_t cnt = 0;
-    for (uint32_t base = 0; base < sarea; base += 32) {
-      const uint32_t k = base + lane;
-      const bool keep =
-          k < sarea && (!stest || tile_can_contribute(spx, spy, sa, sb, sc, sna, snc, st, sx0 + k % sw, sy0 + k / sw));
-      cnt += __popc(__ballot_sync(0xffffffffu, keep));
-    }
-    if (lane == src) kept = cnt;
-  }
+  // rectangles too large for a mask are only counted here
+  walk_large_rects(active && !small, px, py, cd, [&](int src) {
+    return [&, src](uint32_t done, bool, unsigned votes, uint32_t, uint32_t) {
+      if (lane == src) kept = done + __popc(votes);
+    };
+  });
   return kept;
 }
 
@@ -741,16 +789,13 @@ __global__ void __launch_bounds__(256) emit_instances_kernel(int P, const float4
   uint32_t off = end - n;
   if ((int64_t)end > capacity) return;  // host reports GSB_ERR_WORKSPACE
   const float4 A = recA[idx];
-  const float4 B = recB[idx];
-  TileRect rc = tile_rect(A.x, A.y, radii[idx], gx, gy);
+  const Candidate cd =
+      make_candidate(A.x, A.y, radii[idx], recB[idx], A.w, gx, gy, (flags & GSB_RASTER_EXACT_TILE_CULL) != 0);
+  const Footprint& fp = cd.fp;
   const uint32_t depth_bits = __float_as_uint(A.z);
-  const bool exact = flags & GSB_RASTER_EXACT_TILE_CULL;
-  const Footprint fp = make_footprint(B.x, B.y, B.z, exact ? 2.f * logf(255.f * A.w) : 0.f);
-  const bool test = exact && !fp.degenerate;
-  if (exact) rc = shrink_rect(rc, A.x, A.y, fp);
-  for (uint32_t ty = rc.y0; ty < rc.y1; ++ty)
-    for (uint32_t tx = rc.x0; tx < rc.x1; ++tx) {
-      if (test && !tile_can_contribute(A.x, A.y, fp.a, fp.b, fp.c, fp.nb_a, fp.nb_c, fp.two_tau, tx, ty)) continue;
+  for (uint32_t ty = cd.rc.y0; ty < cd.rc.y1; ++ty)
+    for (uint32_t tx = cd.rc.x0; tx < cd.rc.x1; ++tx) {
+      if (cd.test && !tile_can_contribute(A.x, A.y, fp.a, fp.b, fp.c, fp.nb_a, fp.nb_c, fp.two_tau, tx, ty)) continue;
       if (off >= end) return;
       keys[off] = ((uint64_t)(ty * gx + tx) << 32) | depth_bits;
       vals[off] = (uint32_t)idx;
@@ -914,28 +959,13 @@ __global__ void __launch_bounds__(kEmitThreads) emit_sorted_kernel(int P, const 
   if (!small) mask = 0ull;
   // ---- flattened replay of the stored masks (bits up to the highest kept tile of each rectangle)
   const uint32_t cand = small ? 64u - (uint32_t)__clzll((long long)mask) : 0u;
-  uint32_t incl = cand;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const uint32_t v = __shfl_up_sync(0xffffffffu, incl, o);
-    if (lane >= o) incl += v;
-  }
+  const uint32_t incl = warp_inclusive_sum(cand);
   const uint32_t excl = incl - cand;
   const uint32_t total = __shfl_sync(0xffffffffu, incl, 31);
   const uint32_t mlo = (uint32_t)mask, mhi = (uint32_t)(mask >> 32);
   for (uint32_t w0 = 0; w0 < total; w0 += 32) {
     const uint32_t fidx = w0 + lane;
-    int lo = 0, hi = 31;  // the owner of a valid slot is one of the 32 lanes: 5 halvings settle it
-#pragma unroll
-    for (int step = 0; step < 5; ++step) {
-      const int mid = (lo + hi) >> 1;
-      const uint32_t v = __shfl_sync(0xffffffffu, incl, mid);
-      if (v <= fidx)
-        lo = mid + 1;
-      else
-        hi = mid;
-    }
-    const int owner = lo;
+    const int owner = slot_owner(incl, fidx);
     const uint32_t olo = __shfl_sync(0xffffffffu, mlo, owner), ohi = __shfl_sync(0xffffffffu, mhi, owner);
     const uint32_t orect = __shfl_sync(0xffffffffu, rect, owner), oex = __shfl_sync(0xffffffffu, excl, owner);
     const uint32_t ooff = __shfl_sync(0xffffffffu, off, owner), ogid = __shfl_sync(0xffffffffu, gid, owner);
@@ -944,10 +974,9 @@ __global__ void __launch_bounds__(kEmitThreads) emit_sorted_kernel(int P, const 
       const uint64_t om = ((uint64_t)ohi << 32) | olo;
       if ((om >> kk) & 1ull) {
         const uint32_t ordinal = (uint32_t)__popcll(om & ((1ull << kk) - 1ull));
-        const uint32_t ow = (orect >> 26) + 1u;
-        // kk / ow for kk < 64, ow <= 64: (kk + 0.5) / ow is never within rounding distance of an integer
-        const uint32_t row = (uint32_t)__float2int_rd(__fdividef((float)kk + 0.5f, (float)ow));
-        const uint32_t tile = (((orect >> 13) & 0x1fffu) + row) * gx + (orect & 0x1fffu) + (kk - row * ow);
+        const uint3 r = unpack_rect(orect);
+        const uint2 slot = rect_slot(kk, r.z);
+        const uint32_t tile = (r.y + slot.y) * gx + r.x + slot.x;
         const uint32_t dst = ooff + ordinal;
         if ((int64_t)dst < cap) {
           tile_keys[dst] = tile;
@@ -958,54 +987,25 @@ __global__ void __launch_bounds__(kEmitThreads) emit_sorted_kernel(int P, const 
     }
   }
   // ---- rectangles without a mask: re-test, whole warp per Gaussian, ordered by ballot
-  const bool exact = (flags & GSB_RASTER_EXACT_TILE_CULL) != 0;
   float4 A = make_float4(0.f, 0.f, 0.f, 0.f);
-  TileRect rc{0, 0, 0, 0};
-  uint32_t w = 0, area = 0;
-  Footprint fp = make_footprint(1.f, 0.f, 1.f, 0.f);
-  bool test = false;
+  Candidate cd = no_candidate();
   if (active && !small) {
     A = recA[gid];
-    rc = tile_rect(A.x, A.y, radii[gid], gx, gy);
-    if (exact) {
-      const float4 B = recB[gid];
-      fp = make_footprint(B.x, B.y, B.z, 2.f * logf(255.f * A.w));
-      test = !fp.degenerate;
-      rc = shrink_rect(rc, A.x, A.y, fp);
-    }
-    w = rc.x1 - rc.x0;
-    area = w * (rc.y1 - rc.y0);
+    cd = make_candidate(A.x, A.y, radii[gid], recB[gid], A.w, gx, gy, (flags & GSB_RASTER_EXACT_TILE_CULL) != 0);
   }
   const uint32_t lt_mask = (1u << lane) - 1u;
-  unsigned todo = __ballot_sync(0xffffffffu, active && !small);
-  while (todo) {
-    const int src = __ffs(todo) - 1;
-    todo &= todo - 1;
-    const float spx = __shfl_sync(0xffffffffu, A.x, src), spy = __shfl_sync(0xffffffffu, A.y, src);
-    const float sa = __shfl_sync(0xffffffffu, fp.a, src), sb = __shfl_sync(0xffffffffu, fp.b, src);
-    const float sc = __shfl_sync(0xffffffffu, fp.c, src), st = __shfl_sync(0xffffffffu, fp.two_tau, src);
-    const float sna = __shfl_sync(0xffffffffu, fp.nb_a, src), snc = __shfl_sync(0xffffffffu, fp.nb_c, src);
-    const bool stest = __shfl_sync(0xffffffffu, (int)test, src) != 0;
-    const uint32_t sx0 = __shfl_sync(0xffffffffu, rc.x0, src), sy0 = __shfl_sync(0xffffffffu, rc.y0, src);
-    const uint32_t sw = __shfl_sync(0xffffffffu, w, src), sarea = __shfl_sync(0xffffffffu, area, src);
+  walk_large_rects(active && !small, A.x, A.y, cd, [&](int src) {
     const uint32_t soff = __shfl_sync(0xffffffffu, off, src), sgid = __shfl_sync(0xffffffffu, gid, src);
-    uint32_t done = 0;
-    for (uint32_t base = 0; base < sarea; base += 32) {
-      const uint32_t kk = base + lane;
-      const uint32_t tx = sx0 + kk % sw, ty = sy0 + kk / sw;
-      const bool keep = kk < sarea && (!stest || tile_can_contribute(spx, spy, sa, sb, sc, sna, snc, st, tx, ty));
-      const unsigned votes = __ballot_sync(0xffffffffu, keep);
-      if (keep) {
-        const uint32_t dst = soff + done + __popc(votes & lt_mask);
-        if ((int64_t)dst < cap) {
-          tile_keys[dst] = ty * gx + tx;
-          tile_vals[dst] = sgid;
-          tally(ty * gx + tx);
-        }
+    return [&, soff, sgid](uint32_t done, bool keep, unsigned votes, uint32_t tx, uint32_t ty) {
+      if (!keep) return;
+      const uint32_t dst = soff + done + __popc(votes & lt_mask);
+      if ((int64_t)dst < cap) {
+        tile_keys[dst] = ty * gx + tx;
+        tile_vals[dst] = sgid;
+        tally(ty * gx + tx);
       }
-      done += __popc(votes);
-    }
-  }
+    };
+  });
   __syncthreads();
   for (int p = 0; p < hist_passes; ++p) {
     const uint32_t c = shist[p][threadIdx.x];
@@ -1571,6 +1571,19 @@ Workspace carve(void* base, int32_t P, int32_t W, int32_t H, int64_t R) {
 
 bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
+// Zeroes every eye's counters and runs the preprocess pass over the pp.P Gaussians.
+template <int kEyes, int kMinBlocks>
+int preprocess(const PreParams& pp, cudaStream_t stream, bool dbg) {
+  for (int e = 0; e < kEyes; ++e)
+    GSB_CUDA_OK(cudaMemsetAsync(pp.eye[e].counters, 0, 8 * sizeof(unsigned long long), stream));
+  {
+    StageTimer tm(kStPreprocess, stream);
+    preprocess_kernel<kEyes, kMinBlocks><<<(pp.P + kPreThreads - 1) / kPreThreads, kPreThreads, 0, stream>>>(pp);
+  }
+  count_launch();
+  return check_launch(kEyes == 2 ? "preprocess_kernel<2>" : "preprocess_kernel", stream, dbg);
+}
+
 }  // namespace
 }  // namespace gsb
 
@@ -1654,8 +1667,8 @@ constexpr uint32_t kRasterFlags = GSB_RASTER_EXACT_TILE_CULL | GSB_RASTER_NO_TMA
 static int validate_frame(const GsbRasterArgs* a, Frame& f) {
   if (!a) return fail(GSB_ERR_INVALID, "args is NULL");
   if (a->P < 0 || a->width <= 0 || a->height <= 0) return fail(GSB_ERR_INVALID, "bad P / image size");
-  if (a->width > 8191 * kTile || a->height > 8191 * kTile)  // packed candidate rectangles hold 13-bit tile coordinates
-    return fail(GSB_ERR_INVALID, "image side exceeds %d pixels", 8191 * kTile);
+  constexpr int kMaxSide = (int)kRectCoordMax * kTile;  // packed candidate rectangles hold kRectCoordBits-bit tile coordinates
+  if (a->width > kMaxSide || a->height > kMaxSide) return fail(GSB_ERR_INVALID, "image side exceeds %d pixels", kMaxSide);
   if (!a->out_color || !a->background || !a->viewmatrix || !a->projmatrix || !a->cam_pos)
     return fail(GSB_ERR_INVALID, "out_color, background, viewmatrix, projmatrix and cam_pos are required");
   // DGR/diff_gaussian_rasterization/__init__.py:191-195
@@ -1906,14 +1919,7 @@ int gsb_raster_forward(const GsbRasterArgs* a, void* stream_v) {
   fill_eye(f, pp.eye[0]);
   pp.eye[1] = pp.eye[0];
   pp.binned = f.use_cub ? 0 : 1;
-  GSB_CUDA_OK(cudaMemsetAsync(f.ws.counters, 0, 8 * sizeof(unsigned long long), stream));
-  const int pre_blocks = (a->P + kPreThreads - 1) / kPreThreads;
-  {
-    StageTimer tm(kStPreprocess, stream);
-    preprocess_kernel<1, 6><<<pre_blocks, kPreThreads, 0, stream>>>(pp);
-  }
-  count_launch();
-  if ((rc = check_launch("preprocess_kernel", stream, f.dbg))) return rc;
+  if ((rc = preprocess<1, 6>(pp, stream, f.dbg))) return rc;
   if (f.use_cub) return cub_path(f, stream);
   // ---- default pipeline: depth-sort P, emit in that order, stable split by tile; nothing waits
   const uint32_t* ids_sorted = nullptr;
@@ -1949,16 +1955,8 @@ int gsb_raster_forward_pair(const GsbRasterArgs* left, const GsbRasterArgs* righ
   pp.binned = 1;
   const bool shared = (left->flags & GSB_RASTER_PAIR_SHARED_DEPTH) != 0;
   pp.shared_depth = shared ? 1 : 0;
-  GSB_CUDA_OK(cudaMemsetAsync(fl.ws.counters, 0, 8 * sizeof(unsigned long long), sl));
-  GSB_CUDA_OK(cudaMemsetAsync(fr.ws.counters, 0, 8 * sizeof(unsigned long long), sl));
-  const int pre_blocks = (left->P + kPreThreads - 1) / kPreThreads;
-  {
-    StageTimer tm(kStPreprocess, sl);
-    // 5 CTAs per SM: measured on C1 at 0.194 ms (96 registers, 48 B of spills) vs 0.209 ms at 4 (114 registers, no spills)
-    preprocess_kernel<2, 5><<<pre_blocks, kPreThreads, 0, sl>>>(pp);
-  }
-  count_launch();
-  if ((rc = check_launch("preprocess_kernel<2>", sl, fl.dbg))) return rc;
+  // 5 CTAs per SM: measured on C1 at 0.194 ms (96 registers, 48 B of spills) vs 0.209 ms at 4 (114 registers, no spills)
+  if ((rc = preprocess<2, 5>(pp, sl, fl.dbg))) return rc;
   const uint32_t* ids_l = nullptr;
   const uint32_t* ids_r = nullptr;
   if (shared) {  // one depth order for both eyes
