@@ -254,7 +254,9 @@ def registration_icp(source, target, threshold, init=None, with_scaling=True, re
     moments = _Moments(dev)
 
     def result():
-        if grid is not None and n:
+        if grid is None:  # an empty target: no correspondences, and no target rows for the moments to read
+            return np.zeros(12), 0, 0.0, 0.0
+        if n:
             with torch.cuda.device(dev):
                 _lib.check(_lib.lib().gsb_eval_icp_correspond(C.byref(grid.desc), ptr(pcd), n, float(threshold), ptr(idx),
                                                               ptr(d2), _stream(dev)))
