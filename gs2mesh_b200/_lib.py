@@ -107,6 +107,12 @@ SIGNATURES = {
     "gsb_eval_mask_dilate_disk":(C.c_int, [_vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _vp, _vp, _vp]),
     "gsb_eval_cull_vertices_by_masks": (C.c_int, [_vp, C.c_int64, _vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                                   _vp, _vp, _vp]),
+    "gsb_eval_triangle_areas": (C.c_int, [_vp, C.c_int64, _vp, C.c_int64, _vp, _vp]),
+    "gsb_eval_sample_uniform": (C.c_int, [_vp, C.c_int64, _vp, C.c_int64, _vp, _vp, C.c_int64, _vp, _vp]),
+    "gsb_eval_poisson_neighbours": (C.c_int, [C.POINTER(GsbPointGrid), C.c_double, C.c_double, _vp, _vp, _vp, _vp, _vp]),
+    "gsb_eval_poisson_eliminate": (C.c_int, [_vp, _vp, _vp, C.c_int64, _vp, _vp, _vp, _vp, C.POINTER(C.c_int32), _vp]),
+    "gsb_eval_visibility": (C.c_int, [_vp, C.c_int64, C.POINTER(C.c_double), C.c_double, C.POINTER(C.c_int32), _vp, _vp,
+                                      _vp]),
     "gsb_stereo_pack_inputs": (C.c_int, [_vp, _vp, C.c_int32, C.c_int32, _vp, _vp]),
     "gsb_stereo_disparities": (C.c_int, [_vp, _vp, C.c_int32, C.c_int32, C.c_float, _vp, _vp, _vp]),
     "gsb_stereo_occlusion_depth": (C.c_int, [_vp, _vp, C.c_int32, C.c_int32, C.c_int64, C.c_double, C.c_float, _vp, _vp, _vp]),

@@ -217,11 +217,20 @@ def read_point_cloud_ply(path):
     return np.stack([v["x"], v["y"], v["z"]], axis=1).astype(np.float64)
 
 
-def read_triangle_mesh_ply(path):
-    """o3d.io.read_triangle_mesh(path) vertices / triangles (eval.py:46-49): (float64 [N,3], int64 [M,3])."""
+def read_triangle_mesh_ply(path, with_colors=False):
+    """o3d.io.read_triangle_mesh(path) vertices / triangles (eval.py:46-49): (float64 [N,3], int64 [M,3]).  with_colors
+    adds a third item, the vertex colours as Open3D reads uchar red / green / blue (value / 255, float64 [N,3]), or None
+    when the file has none."""
     v, tris = _read_vertex_table(path, with_faces=True)
     xyz = np.stack([v["x"], v["y"], v["z"]], axis=1).astype(np.float64)
-    return xyz, (np.zeros((0, 3), np.int64) if tris is None else tris)
+    tris = np.zeros((0, 3), np.int64) if tris is None else tris
+    if not with_colors:
+        return xyz, tris
+    names = v.dtype.names
+    colors = None
+    if all(c in names for c in ("red", "green", "blue")):
+        colors = np.stack([v["red"], v["green"], v["blue"]], axis=1).astype(np.float64) / 255.0
+    return xyz, tris, colors
 
 
 def write_point_cloud_ply(path, points, colors=None):

@@ -424,6 +424,48 @@ int gsb_eval_cull_vertices_by_masks(const double* vertices, int64_t n_vertices, 
                                     int32_t image_width, int32_t image_height, int32_t mask_width, int32_t mask_height,
                                     const uint32_t* packed_masks, uint8_t* keep, void* stream);
 
+/* MobileBrick evaluation (evaluation/MobileBrick/eval_code/evaluate.py:34-108), restating Open3D 0.17's
+ * TriangleMesh::GetSurfaceArea, SamplePointsUniformlyImpl and SamplePointsPoissonDisk and the reference's grid_sample
+ * visibility test; DESIGN.md section 7e gives each operation order.  vertices: device double [n_vertices,3]; triangles:
+ * device int64 [n_triangles,3].
+ *   gsb_eval_triangle_areas     areas[t] = 0.5 * |(p0 - p1) x (p0 - p2)|, the norm as sqrt((x*x + y*y) + z*z).
+ *   gsb_eval_sample_uniform     sample j of n_samples lies on the triangle t with bounds[t] <= j < bounds[t+1] (bounds:
+ *                               device int64 [n_triangles+1], nondecreasing, bounds[0] = 0); with r1 = variates[2j],
+ *                               r2 = variates[2j+1] (device double [2*n_samples]), a = 1 - sqrt(r1), b = sqrt(r1)*(1 - r2),
+ *                               c = sqrt(r1)*r2, samples[j] = (a*p0 + b*p1) + c*p2.  Samples j >= bounds[n_triangles] are
+ *                               (0,0,0).  n_triangles >= 1.
+ *   gsb_eval_poisson_neighbours the radius neighbours of each grid point p: every q != p with ((dx*dx)+dy*dy)+dz*dz <
+ *                               r_max*r_max (dx = p.x - q.x).  Needs grid->cell > r_max and fewer than 2^31 points.  With
+ *                               offsets NULL it writes counts[p] (device int64 [n_points]); with offsets (device int64
+ *                               [n_points+1], the exclusive scan of the counts and the total) it writes each list at
+ *                               neighbours + offsets[p] (device int32), sorted by (squared distance, index), and terms[k]
+ *                               = (1 - max(sqrt(d2), r_min)/r_max)^8, the power as three squarings (device double).
+ *                               The emit call reads offsets[n_points] back: it SYNCHRONISES the stream.
+ *   gsb_eval_poisson_eliminate  weighted sample elimination as rounds: a point's weight is the sum of its live neighbours'
+ *                               terms in list order; each round deletes every live point whose key (weight, index) exceeds
+ *                               the keys of all its live neighbours.  Runs until every point is deleted: weight (device
+ *                               double [n_points]) then holds each point's removal key, round_of (device int32 [n_points])
+ *                               the round that deleted it (from 1).  Open3D's loop keeps the number_of_points points of
+ *                               smallest (weight, index).  Reads the live count every 4 rounds: SYNCHRONISES the stream.
+ *                               counters: device uint32[4] scratch; host_live: pinned host uint32[4]; rounds (may be NULL)
+ *                               receives the number of rounds.
+ *   gsb_eval_visibility         keep[i] = 1 iff grid_sample(volume, g, nearest, zeros, align_corners=True) > 0 for
+ *                               g = fp32(((((p - min_pts)/voxel_size) / (res - 1)) * 2) - 1) (fp64 until the rounding), axes
+ *                               reordered to (z, y, x); volume: device uint8 [res0][res1][res2], nonzero where the
+ *                               reference's float volume is > 0.  min_pts: host double [3]; resolution: host int32 [3], each
+ *                               >= 2. */
+int gsb_eval_triangle_areas(const double* vertices, int64_t n_vertices, const int64_t* triangles, int64_t n_triangles,
+                            double* areas, void* stream);
+int gsb_eval_sample_uniform(const double* vertices, int64_t n_vertices, const int64_t* triangles, int64_t n_triangles,
+                            const int64_t* bounds, const double* variates, int64_t n_samples, double* samples, void* stream);
+int gsb_eval_poisson_neighbours(const GsbPointGrid* grid, double r_max, double r_min, int64_t* counts,
+                                const int64_t* offsets, int32_t* neighbours, double* terms, void* stream);
+int gsb_eval_poisson_eliminate(const int64_t* offsets, const int32_t* neighbours, const double* terms, int64_t n_points,
+                               double* weight, int32_t* round_of, uint32_t* counters, uint32_t* host_live, int32_t* rounds,
+                               void* stream);
+int gsb_eval_visibility(const double* vertices, int64_t n_vertices, const double* min_pts, double voxel_size,
+                        const int32_t* resolution, const uint8_t* volume, uint8_t* keep, void* stream);
+
 /* ------------------------------------------------------------------------------------------
  * Stereo stage (gs2mesh_utils/stereo_utils.py:82-179) around the caller's disparity model.
  * ------------------------------------------------------------------------------------------
