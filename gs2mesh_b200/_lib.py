@@ -91,6 +91,10 @@ SIGNATURES = {
     "gsb_mesh_emit": (C.c_int, [_vp, C.POINTER(C.c_int32), _vp, C.c_uint32, _vp, _vp, _vp]),
     "gsb_mesh_vertices": (C.c_int, [_vp, C.POINTER(C.c_int32), _vp, C.c_int64, _vp, _vp, _vp]),
     "gsb_mesh_vertex_normals": (C.c_int, [_vp, C.c_int64, _vp, C.c_int64, _vp, _vp, _vp, _vp]),
+    "gsb_mesh_cluster_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int64]),
+    "gsb_mesh_clusters": (C.c_int, [_vp, C.c_int64, C.c_int64, _vp, _vp, C.c_size_t, _vp, _vp, _vp, _vp, _vp]),
+    "gsb_mesh_remove_small_clusters": (C.c_int, [_vp, C.c_int64, C.c_int64, _vp, _vp, C.c_double, _vp, C.c_size_t, _vp, _vp,
+                                                 _vp, _vp]),
     "gsb_eval_sample_count": (C.c_int, [_vp, C.c_int64, _vp, C.c_int64, C.c_double, _vp, _vp]),
     "gsb_eval_sample_emit": (C.c_int, [_vp, C.c_int64, _vp, C.c_int64, C.c_double, _vp, _vp, _vp]),
     "gsb_eval_grid_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int64]),

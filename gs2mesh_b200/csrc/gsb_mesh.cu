@@ -9,6 +9,14 @@
 // in shared memory; a count pass and an emit pass write three 64-bit edge keys per triangle
 // (key = global voxel index * 3 + axis); the caller uniques the keys (vertex ids) and a vertex
 // kernel evaluates positions / colours per unique edge in fp64 with Open3D's formulas.
+//
+// Cluster cleaning (tsdf_utils.py:122-142, TriangleMesh::ClusterConnectedTriangles + removal of small clusters and
+// unreferenced vertices): triangles sharing an edge are grouped by a radix sort of 64-bit edge keys, joined by a
+// lock-free union-find whose roots are the smallest triangle of each cluster, and numbered by an exclusive scan of the
+// root flags -- the order Open3D's BFS loop and scipy's connected_components number them in.
+#include <cub/cub.cuh>
+#include <cuda/atomic>
+
 #include "gs2mesh_b200.h"
 #include "gsb_common.h"
 #include "gsb_mc_tables.h"
@@ -231,6 +239,256 @@ int window_check(const char* who, const int32_t* w) {
   return GSB_OK;
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// Edge-connected triangle clusters.  Union-find over triangle ids in the style of ECL-CC: a larger root is always hooked
+// under a smaller one with atomicCAS, so parent[t] <= t holds at every moment and the surviving root of a cluster is its
+// smallest triangle.  Parents are read with relaxed atomic loads; finds halve the path they walk.  Only roots are ever
+// CAS'd and a non-root never becomes a root again, so a path-halving store (an ancestor into a non-root) cannot undo a
+// hook.
+// ---------------------------------------------------------------------------------------------------------------------
+using ParentRef = cuda::atomic_ref<int, cuda::thread_scope_device>;
+
+__device__ __forceinline__ int uf_load(int* parent, int x) { return ParentRef(parent[x]).load(cuda::memory_order_relaxed); }
+
+__device__ __forceinline__ int uf_find(int* parent, int x) {
+  int p = uf_load(parent, x);
+  while (p != x) {
+    const int gp = uf_load(parent, p);
+    if (gp != p) ParentRef(parent[x]).store(gp, cuda::memory_order_relaxed);
+    x = gp;
+    p = uf_load(parent, x);
+  }
+  return x;
+}
+
+__device__ __forceinline__ void uf_union(int* parent, int a, int b) {
+  a = uf_find(parent, a);
+  b = uf_find(parent, b);
+  while (a != b) {
+    if (a < b) {
+      const int s = a;
+      a = b;
+      b = s;
+    }
+    const int old = atomicCAS(&parent[a], a, b);  // hook the larger root under the smaller
+    if (old == a) return;
+    a = uf_find(parent, old);  // a was hooked elsewhere in the meantime
+    b = uf_find(parent, b);
+  }
+}
+
+// Three (key, triangle) pairs per triangle, edges (a,b), (b,c), (c,a) in that order; key = min*(n_vertices+1) + max,
+// the host's key (mesh.py) and Open3D's GetEdgeToTrianglesMap.  Degenerate edges (a,a) get keys like any other.
+__global__ void __launch_bounds__(256) cluster_edge_keys_kernel(const long long* __restrict__ tris, int nt,
+                                                                unsigned long long stride, unsigned long long* __restrict__ keys,
+                                                                uint32_t* __restrict__ owner, int* __restrict__ parent) {
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= nt) return;
+  const long long v[3] = {tris[3 * (size_t)t], tris[3 * (size_t)t + 1], tris[3 * (size_t)t + 2]};
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    const long long a = v[k], b = v[(k + 1) % 3];
+    const unsigned long long lo = (unsigned long long)(a < b ? a : b), hi = (unsigned long long)(a < b ? b : a);
+    keys[(size_t)k * nt + t] = lo * stride + hi;
+    owner[(size_t)k * nt + t] = (uint32_t)t;
+  }
+  parent[t] = t;
+}
+
+// Neighbours in the sorted key array with equal keys share an edge: joining each with its predecessor joins every run.
+__global__ void __launch_bounds__(256) cluster_union_kernel(const unsigned long long* __restrict__ keys,
+                                                            const uint32_t* __restrict__ owner, long long n, int* parent) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x + 1;
+  if (i >= n || keys[i] != keys[i - 1]) return;
+  uf_union(parent, (int)owner[i], (int)owner[i - 1]);
+}
+
+// After every hook: parent[t] = its root, root_flag[t] = 1 for the roots.  The walk here does not halve: a halving
+// store into parent[x] could land after thread x wrote its root there and leave x pointing at a non-root.  Each
+// parent[t] is written once, by thread t, and every value a walk can read is an ancestor, so every walk ends at the root.
+__global__ void __launch_bounds__(256) cluster_compress_kernel(int* parent, int nt, int* __restrict__ root_flag) {
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= nt) return;
+  int r = t, p = uf_load(parent, t);
+  while (p != r) {
+    r = p;
+    p = uf_load(parent, r);
+  }
+  ParentRef(parent[t]).store(r, cuda::memory_order_relaxed);
+  root_flag[t] = r == t;
+}
+
+// label[t] = the rank of t's root among the roots (clusters numbered by their smallest triangle); counts by integer
+// atomics (exact, so the same on every run); the last thread writes the number of clusters.
+__global__ void __launch_bounds__(256) cluster_label_kernel(const int* __restrict__ parent, const int* __restrict__ root_flag,
+                                                            const int* __restrict__ rank, int nt, long long* __restrict__ labels,
+                                                            unsigned long long* counts, long long* __restrict__ n_clusters,
+                                                            uint32_t* __restrict__ label32) {
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= nt) return;
+  const int l = rank[parent[t]];
+  labels[t] = l;
+  if (label32) label32[t] = (uint32_t)l;
+  atomicAdd(&counts[l], 1ull);
+  if (t == nt - 1) *n_clusters = (long long)rank[t] + root_flag[t];
+}
+
+// 0.5 * ||(v1-v0) x (v2-v0)|| with numpy's roundings: np.cross computes each component as one product minus another,
+// np.linalg.norm(axis=1) as sqrt((x*x + y*y) + z*z); no FMA contraction.
+__global__ void __launch_bounds__(256) triangle_area_kernel(const double* __restrict__ xyz, const long long* __restrict__ tris,
+                                                            int nt, double* __restrict__ area) {
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= nt) return;
+  const long long i0 = tris[3 * (size_t)t], i1 = tris[3 * (size_t)t + 1], i2 = tris[3 * (size_t)t + 2];
+  const double x0 = xyz[3 * i0], y0 = xyz[3 * i0 + 1], z0 = xyz[3 * i0 + 2];
+  const double ax = __dsub_rn(xyz[3 * i1], x0), ay = __dsub_rn(xyz[3 * i1 + 1], y0), az = __dsub_rn(xyz[3 * i1 + 2], z0);
+  const double bx = __dsub_rn(xyz[3 * i2], x0), by = __dsub_rn(xyz[3 * i2 + 1], y0), bz = __dsub_rn(xyz[3 * i2 + 2], z0);
+  const double cx = __dsub_rn(__dmul_rn(ay, bz), __dmul_rn(az, by));
+  const double cy = __dsub_rn(__dmul_rn(az, bx), __dmul_rn(ax, bz));
+  const double cz = __dsub_rn(__dmul_rn(ax, by), __dmul_rn(ay, bx));
+  area[t] = __dmul_rn(0.5, __dsqrt_rn(__dadd_rn(__dadd_rn(__dmul_rn(cx, cx), __dmul_rn(cy, cy)), __dmul_rn(cz, cz))));
+}
+
+// One warp per cluster sums its triangles' areas (sorted by label, ascending triangle id inside a label) in a fixed
+// order: lane-strided partial sums, then a fixed butterfly.  No floating-point atomics, so the bits repeat run to run.
+__global__ void __launch_bounds__(256) cluster_area_sum_kernel(const double* __restrict__ sorted_area,
+                                                               const long long* __restrict__ offsets,
+                                                               const unsigned long long* __restrict__ counts, int nt,
+                                                               double* __restrict__ cluster_area) {
+  const long long c = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (c >= nt) return;
+  const long long begin = offsets[c], n = (long long)counts[c];
+  double s = 0.0;
+  for (long long j = lane; j < n; j += 32) s = __dadd_rn(s, sorted_area[begin + j]);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) s = __dadd_rn(s, __shfl_xor_sync(0xffffffffu, s, o));
+  if (lane == 0) cluster_area[c] = s;
+}
+
+// keep[t] = !(counts[labels[t]] < threshold), the comparison numpy makes between int64 counts and a float threshold.
+__global__ void __launch_bounds__(256) cluster_keep_kernel(const long long* __restrict__ labels,
+                                                           const long long* __restrict__ counts, int nt, double threshold,
+                                                           int* __restrict__ keep) {
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= nt) return;
+  keep[t] = !((double)counts[labels[t]] < threshold);
+}
+
+__global__ void __launch_bounds__(256) mark_referenced_kernel(const long long* __restrict__ tris, const int* __restrict__ keep,
+                                                              int nt, int* __restrict__ referenced) {
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= nt || !keep[t]) return;
+#pragma unroll
+  for (int k = 0; k < 3; ++k) referenced[tris[3 * (size_t)t + k]] = 1;
+}
+
+__global__ void __launch_bounds__(256) remap_triangles_kernel(const long long* __restrict__ tris, const int* __restrict__ keep,
+                                                              const int* __restrict__ tri_pos, const int* __restrict__ new_id,
+                                                              int nt, long long* __restrict__ out_tris) {
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= nt || !keep[t]) return;
+  const size_t o = 3 * (size_t)tri_pos[t];
+#pragma unroll
+  for (int k = 0; k < 3; ++k) out_tris[o + k] = new_id[tris[3 * (size_t)t + k]];
+}
+
+__global__ void __launch_bounds__(256) kept_vertices_kernel(const int* __restrict__ referenced, const int* __restrict__ new_id,
+                                                            int nv, long long* __restrict__ vertex_ids) {
+  const int v = blockIdx.x * blockDim.x + threadIdx.x;
+  if (v < nv && referenced[v]) vertex_ids[new_id[v]] = v;
+}
+
+__global__ void clean_sizes_kernel(const int* __restrict__ keep, const int* __restrict__ tri_pos, int nt,
+                                   const int* __restrict__ referenced, const int* __restrict__ new_id, int nv,
+                                   long long* __restrict__ sizes) {
+  sizes[0] = nt ? (long long)tri_pos[nt - 1] + keep[nt - 1] : 0;
+  sizes[1] = nv ? (long long)new_id[nv - 1] + referenced[nv - 1] : 0;
+}
+
+inline unsigned blocks_of(long long n, int per_block = 256) { return (unsigned)((n + per_block - 1) / per_block); }
+
+inline int bits_of(unsigned long long max_value) {
+  int b = 0;
+  while (b < 64 && (max_value >> b) != 0) ++b;
+  return b;
+}
+
+// Ids are 32-bit inside the kernels; edge keys min*(n_vertices+1) + max then fit 62 bits.
+constexpr int64_t kMaxClusterIds = 2147483647;
+
+// Workspace layout of the two cluster entries (each carves its own regions from the start of the block); with a NULL
+// base only `total` is meaningful.
+struct ClusterWork {
+  unsigned long long* keys;  // [2][3 nt] edge keys (DoubleBuffer); later [2 nt] sorted-by-label areas + [nt] offsets
+  uint32_t* owner;           // [2][3 nt] triangle of each key (DoubleBuffer); later [2 nt] labels as sort keys
+  int* parent;               // [nt]
+  int* flag;                 // [nt]
+  int* rank;                 // [nt]
+  void* tmp;
+  size_t tmp_bytes, total;
+};
+struct CleanWork {
+  int *keep, *tri_pos, *referenced, *new_id;  // [nt], [nt], [nv], [nv]
+  void* tmp;
+  size_t tmp_bytes, total;
+};
+
+size_t cub_tmp_bytes(int64_t nt, int64_t nv) {
+  const long long n3 = 3 * nt;
+  size_t a = 0, b = 0, c = 0, d = 0, e = 0;
+  cub::DoubleBuffer<unsigned long long> k(nullptr, nullptr);
+  cub::DoubleBuffer<uint32_t> o(nullptr, nullptr);
+  cub::DeviceRadixSort::SortPairs(nullptr, a, k, o, n3);
+  cub::DoubleBuffer<uint32_t> lk(nullptr, nullptr);
+  cub::DoubleBuffer<double> av(nullptr, nullptr);
+  cub::DeviceRadixSort::SortPairs(nullptr, b, lk, av, (long long)nt);
+  cub::DeviceScan::ExclusiveSum(nullptr, c, (int*)nullptr, (int*)nullptr, (long long)nt);
+  cub::DeviceScan::ExclusiveSum(nullptr, d, (int*)nullptr, (int*)nullptr, (long long)nv);
+  cub::DeviceScan::ExclusiveSum(nullptr, e, (unsigned long long*)nullptr, (long long*)nullptr, (long long)nt);
+  size_t m = a;
+  for (size_t x : {b, c, d, e}) m = x > m ? x : m;
+  return m;
+}
+
+ClusterWork carve_cluster(void* base, int64_t nt, int64_t nv) {
+  Carver c(base);
+  ClusterWork w;
+  w.keys = c.take<unsigned long long>(6 * (size_t)nt);
+  w.owner = c.take<uint32_t>(6 * (size_t)nt);
+  w.parent = c.take<int>((size_t)nt);
+  w.flag = c.take<int>((size_t)nt);
+  w.rank = c.take<int>((size_t)nt);
+  w.tmp_bytes = cub_tmp_bytes(nt, nv);
+  w.tmp = c.take<char>(w.tmp_bytes);
+  w.total = c.total();
+  return w;
+}
+
+CleanWork carve_clean(void* base, int64_t nt, int64_t nv) {
+  Carver c(base);
+  CleanWork w;
+  w.keep = c.take<int>((size_t)nt);
+  w.tri_pos = c.take<int>((size_t)nt);
+  w.referenced = c.take<int>((size_t)nv);
+  w.new_id = c.take<int>((size_t)nv);
+  w.tmp_bytes = cub_tmp_bytes(nt, nv);
+  w.tmp = c.take<char>(w.tmp_bytes);
+  w.total = c.total();
+  return w;
+}
+
+bool cluster_sizes_ok(int64_t nt, int64_t nv) {
+  return nt >= 0 && nv >= 0 && nt <= kMaxClusterIds && nv <= kMaxClusterIds && (nt == 0 || nv > 0);
+}
+
+int cluster_size_error(const char* who, int64_t nt, int64_t nv) {
+  if (nt < 0 || nv < 0) return fail(GSB_ERR_INVALID, "%s: negative size (n_triangles %lld, n_vertices %lld)", who, (long long)nt, (long long)nv);
+  if (nt > 0 && nv == 0 && nt <= kMaxClusterIds) return fail(GSB_ERR_INVALID, "%s: %lld triangles but no vertices", who, (long long)nt);
+  return fail(GSB_ERR_INVALID, "%s: %lld triangles / %lld vertices; triangle and vertex ids are 32-bit (at most %lld each)", who,
+              (long long)nt, (long long)nv, (long long)kMaxClusterIds);
+}
+
 }  // namespace
 }  // namespace gsb
 
@@ -285,6 +543,115 @@ int gsb_mesh_vertex_normals(const double* xyz, int64_t n_vertices, const int64_t
       reinterpret_cast<const long long*>(incidence_offsets), n_vertices, normals);
   count_launch();
   return check_launch("mesh_vertex_normals_kernel", stream, false);
+}
+
+size_t gsb_mesh_cluster_workspace_bytes(int64_t n_triangles, int64_t n_vertices) {
+  if (!cluster_sizes_ok(n_triangles, n_vertices)) return 0;
+  const size_t a = carve_cluster(nullptr, n_triangles, n_vertices).total, b = carve_clean(nullptr, n_triangles, n_vertices).total;
+  return a > b ? a : b;
+}
+
+int gsb_mesh_clusters(const int64_t* triangles, int64_t n_triangles, int64_t n_vertices, const double* vertices, void* workspace,
+                      size_t workspace_bytes, int64_t* labels, int64_t* counts, int64_t* n_clusters, double* cluster_area,
+                      void* stream_v) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
+  if (!cluster_sizes_ok(n_triangles, n_vertices)) return cluster_size_error("mesh_clusters", n_triangles, n_vertices);
+  if (!n_clusters || (n_triangles && (!triangles || !workspace || !labels || !counts || (cluster_area && !vertices))))
+    return fail(GSB_ERR_INVALID, "mesh_clusters: bad arguments");
+  if (n_triangles == 0) {
+    GSB_CUDA_OK(cudaMemsetAsync(n_clusters, 0, sizeof(int64_t), stream));
+    return GSB_OK;
+  }
+  const size_t need = gsb_mesh_cluster_workspace_bytes(n_triangles, n_vertices);
+  if (workspace_bytes < need) return fail(GSB_ERR_WORKSPACE, "mesh_clusters: workspace %zu < %zu bytes", workspace_bytes, need);
+  const int nt = (int)n_triangles;
+  const long long n3 = 3 * (long long)nt;
+  const ClusterWork w = carve_cluster(workspace, n_triangles, n_vertices);
+  const auto* tris = reinterpret_cast<const long long*>(triangles);
+  const unsigned long long stride = (unsigned long long)n_vertices + 1;
+  const int key_bits = bits_of(stride * stride - 1);  // keys < (n_vertices+1)^2
+
+  cluster_edge_keys_kernel<<<blocks_of(nt), 256, 0, stream>>>(tris, nt, stride, w.keys, w.owner, w.parent);
+  count_launch();
+  cub::DoubleBuffer<unsigned long long> keys(w.keys, w.keys + n3);
+  cub::DoubleBuffer<uint32_t> owner(w.owner, w.owner + n3);
+  size_t tmp_bytes = w.tmp_bytes;
+  GSB_CUDA_OK(cub::DeviceRadixSort::SortPairs(w.tmp, tmp_bytes, keys, owner, n3, 0, key_bits, stream));
+  if (n3 > 1) {
+    cluster_union_kernel<<<blocks_of(n3 - 1), 256, 0, stream>>>(keys.Current(), owner.Current(), n3, w.parent);
+    count_launch();
+  }
+  cluster_compress_kernel<<<blocks_of(nt), 256, 0, stream>>>(w.parent, nt, w.flag);
+  count_launch();
+  tmp_bytes = w.tmp_bytes;
+  GSB_CUDA_OK(cub::DeviceScan::ExclusiveSum(w.tmp, tmp_bytes, w.flag, w.rank, (long long)nt, stream));
+  auto* ucounts = reinterpret_cast<unsigned long long*>(counts);
+  GSB_CUDA_OK(cudaMemsetAsync(counts, 0, sizeof(int64_t) * (size_t)nt, stream));
+  // the edge sort's buffers are free from here on: labels as sort keys in `owner`, areas and offsets in `keys`
+  uint32_t* label32 = cluster_area ? w.owner : nullptr;
+  cluster_label_kernel<<<blocks_of(nt), 256, 0, stream>>>(w.parent, w.flag, w.rank, nt, reinterpret_cast<long long*>(labels),
+                                                          ucounts, reinterpret_cast<long long*>(n_clusters), label32);
+  count_launch();
+  if (int rc = check_launch("mesh_clusters", stream, false)) return rc;
+  if (!cluster_area) return GSB_OK;
+
+  auto* area = reinterpret_cast<double*>(w.keys);
+  auto* offsets = reinterpret_cast<long long*>(w.keys + 2 * (size_t)nt);
+  triangle_area_kernel<<<blocks_of(nt), 256, 0, stream>>>(vertices, tris, nt, area);
+  count_launch();
+  cub::DoubleBuffer<uint32_t> by_label(label32, label32 + nt);
+  cub::DoubleBuffer<double> areas(area, area + nt);
+  tmp_bytes = w.tmp_bytes;  // a stable sort: each cluster's areas stay in triangle order
+  GSB_CUDA_OK(cub::DeviceRadixSort::SortPairs(w.tmp, tmp_bytes, by_label, areas, (long long)nt, 0, bits_of((unsigned long long)nt),
+                                              stream));
+  tmp_bytes = w.tmp_bytes;
+  GSB_CUDA_OK(cub::DeviceScan::ExclusiveSum(w.tmp, tmp_bytes, ucounts, offsets, (long long)nt, stream));
+  cluster_area_sum_kernel<<<blocks_of(32 * (long long)nt), 256, 0, stream>>>(areas.Current(), offsets, ucounts, nt, cluster_area);
+  count_launch();
+  return check_launch("mesh_clusters(area)", stream, false);
+}
+
+int gsb_mesh_remove_small_clusters(const int64_t* triangles, int64_t n_triangles, int64_t n_vertices, const int64_t* labels,
+                                   const int64_t* counts, double threshold, void* workspace, size_t workspace_bytes,
+                                   int64_t* out_triangles, int64_t* vertex_ids, int64_t* sizes, void* stream_v) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
+  if (!cluster_sizes_ok(n_triangles, n_vertices)) return cluster_size_error("mesh_remove_small_clusters", n_triangles, n_vertices);
+  if (!sizes || (n_triangles && (!triangles || !labels || !counts || !out_triangles)) ||
+      ((n_triangles || n_vertices) && !workspace) || (n_vertices && !vertex_ids))
+    return fail(GSB_ERR_INVALID, "mesh_remove_small_clusters: bad arguments");
+  const size_t need = gsb_mesh_cluster_workspace_bytes(n_triangles, n_vertices);
+  if ((n_triangles || n_vertices) && workspace_bytes < need)
+    return fail(GSB_ERR_WORKSPACE, "mesh_remove_small_clusters: workspace %zu < %zu bytes", workspace_bytes, need);
+  const int nt = (int)n_triangles, nv = (int)n_vertices;
+  const CleanWork w = carve_clean(workspace, n_triangles, n_vertices);
+  const auto* tris = reinterpret_cast<const long long*>(triangles);
+  size_t tmp_bytes;
+  if (nt) {
+    cluster_keep_kernel<<<blocks_of(nt), 256, 0, stream>>>(reinterpret_cast<const long long*>(labels),
+                                                           reinterpret_cast<const long long*>(counts), nt, threshold, w.keep);
+    count_launch();
+    tmp_bytes = w.tmp_bytes;
+    GSB_CUDA_OK(cub::DeviceScan::ExclusiveSum(w.tmp, tmp_bytes, w.keep, w.tri_pos, (long long)nt, stream));
+  }
+  if (nv) {
+    GSB_CUDA_OK(cudaMemsetAsync(w.referenced, 0, sizeof(int) * (size_t)nv, stream));
+    if (nt) {
+      mark_referenced_kernel<<<blocks_of(nt), 256, 0, stream>>>(tris, w.keep, nt, w.referenced);
+      count_launch();
+    }
+    tmp_bytes = w.tmp_bytes;
+    GSB_CUDA_OK(cub::DeviceScan::ExclusiveSum(w.tmp, tmp_bytes, w.referenced, w.new_id, (long long)nv, stream));
+    kept_vertices_kernel<<<blocks_of(nv), 256, 0, stream>>>(w.referenced, w.new_id, nv, reinterpret_cast<long long*>(vertex_ids));
+    count_launch();
+  }
+  if (nt) {
+    remap_triangles_kernel<<<blocks_of(nt), 256, 0, stream>>>(tris, w.keep, w.tri_pos, w.new_id, nt,
+                                                              reinterpret_cast<long long*>(out_triangles));
+    count_launch();
+  }
+  clean_sizes_kernel<<<1, 1, 0, stream>>>(w.keep, w.tri_pos, nt, w.referenced, w.new_id, nv, reinterpret_cast<long long*>(sizes));
+  count_launch();
+  return check_launch("mesh_remove_small_clusters", stream, false);
 }
 
 }  // extern "C"

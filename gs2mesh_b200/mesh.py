@@ -4,8 +4,10 @@ reference delegates to Open3D's TriangleMesh (lines 108-110 extract / scale / ve
 
 Marching cubes, vertex attributes and vertex normals run on the GPU (gsb_mesh_* in
 include/gs2mesh_b200.h); vertex de-duplication is a sort/unique of 64-bit edge keys (what Open3D
-does with a hash map); connected-component cleaning and PLY writing stay on the host like in
-the reference.
+does with a hash map).  Connected-component cleaning runs on the GPU for a mesh extracted from a
+GPU volume (`TriangleMesh.device` is set) and with numpy / scipy for a mesh built from host arrays;
+both give the same labels, counts and cleaned mesh.  PLY writing stays on the host like in the
+reference.
 """
 from __future__ import annotations
 
@@ -33,7 +35,10 @@ def color_to_uint8(colors):
 class TriangleMesh:
     """Minimal stand-in for open3d.geometry.TriangleMesh (the members tsdf_utils.py touches)."""
 
-    def __init__(self, vertices, triangles, vertex_colors=None, vertex_normals=None):
+    def __init__(self, vertices, triangles, vertex_colors=None, vertex_normals=None, device=None):
+        # the CUDA device a mesh extracted from a GPU volume came from; None for a mesh built from host arrays.  Cluster
+        # cleaning runs there (the arrays themselves are host numpy either way).
+        self.device = None if device is None else torch.device(device)
         self.vertices = np.asarray(vertices, dtype=np.float64).reshape(-1, 3)
         self.triangles = np.asarray(triangles, dtype=np.int64).reshape(-1, 3)
         self.vertex_colors = None if vertex_colors is None else np.asarray(vertex_colors, dtype=np.float64).reshape(-1, 3)
@@ -70,8 +75,33 @@ class TriangleMesh:
             self.vertex_normals = out.cpu().numpy()
         return self
 
+    def _clusters_on_device(self, with_area):
+        """gsb_mesh_clusters on self.device: (device triangles, workspace, labels, counts, n_clusters, cluster areas or
+        None), all enqueued on the device's current stream."""
+        nv, nt = len(self.vertices), len(self.triangles)
+        if nt and (self.triangles.min() < 0 or self.triangles.max() >= nv):
+            raise ValueError("cluster_connected_triangles: triangle vertex index out of range")
+        dev = self.device
+        L = _lib.lib()
+        stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+        tri = torch.as_tensor(self.triangles, dtype=torch.int64).to(dev).contiguous()
+        work = torch.empty(L.gsb_mesh_cluster_workspace_bytes(nt, nv), dtype=torch.uint8, device=dev)
+        labels = torch.empty(nt, dtype=torch.int64, device=dev)
+        counts = torch.empty(nt, dtype=torch.int64, device=dev)
+        n = torch.empty(1, dtype=torch.int64, device=dev)
+        xyz = torch.as_tensor(self.vertices).to(dev).contiguous() if with_area else None
+        area = torch.empty(nt, dtype=torch.float64, device=dev) if with_area else None
+        _lib.check(L.gsb_mesh_clusters(ptr(tri), nt, nv, ptr(xyz), ptr(work), work.numel(), ptr(labels), ptr(counts), ptr(n),
+                                       ptr(area), stream))
+        return tri, work, labels, counts, n, area
+
     # -- tsdf_utils.py:132-133 (TriangleMesh::ClusterConnectedTriangles: triangles sharing an edge)
     def cluster_connected_triangles(self):
+        if self.device is not None:
+            with torch.cuda.device(self.device):
+                _, _, labels, counts, n, area = self._clusters_on_device(with_area=True)
+                k = int(n.item())
+                return labels.cpu().numpy(), counts[:k].cpu().numpy(), area[:k].cpu().numpy()
         from scipy.sparse import coo_matrix
         from scipy.sparse.csgraph import connected_components
 
@@ -96,6 +126,8 @@ class TriangleMesh:
 
     # -- tsdf_utils.py:137-140
     def remove_small_clusters(self, min_triangles):
+        if self.device is not None:
+            return self._remove_small_clusters_on_device(min_triangles)
         labels, counts, _ = self.cluster_connected_triangles()
         keep = ~(counts[labels] < min_triangles) if len(labels) else np.zeros(0, bool)
         tris = self.triangles[keep]
@@ -104,6 +136,25 @@ class TriangleMesh:
         remap = np.cumsum(used) - 1
         pick = lambda a: None if a is None else a[used]
         return TriangleMesh(self.vertices[used], remap[tris], pick(self.vertex_colors), pick(self.vertex_normals))
+
+    def _remove_small_clusters_on_device(self, min_triangles):
+        """remove_small_clusters on self.device: the triangles go up once, the kept triangles (renumbered) and the old ids
+        of the kept vertices come back, and the vertex arrays are gathered where they live."""
+        nv, nt = len(self.vertices), len(self.triangles)
+        with torch.cuda.device(self.device):
+            dev = self.device
+            stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+            tri, work, labels, counts, _, _ = self._clusters_on_device(with_area=False)
+            out_tri = torch.empty(nt, 3, dtype=torch.int64, device=dev)
+            ids = torch.empty(nv, dtype=torch.int64, device=dev)
+            sizes = torch.empty(2, dtype=torch.int64, device=dev)
+            _lib.check(_lib.lib().gsb_mesh_remove_small_clusters(ptr(tri), nt, nv, ptr(labels), ptr(counts), float(min_triangles),
+                                                                 ptr(work), work.numel(), ptr(out_tri), ptr(ids), ptr(sizes),
+                                                                 stream))
+            kt, kv = (int(x) for x in sizes.cpu().tolist())
+            tris, used = out_tri[:kt].cpu().numpy(), ids[:kv].cpu().numpy()
+        pick = lambda a: None if a is None else a[used]
+        return TriangleMesh(self.vertices[used], tris, pick(self.vertex_colors), pick(self.vertex_normals), device=self.device)
 
     # -- o3d.io.write_triangle_mesh(path, mesh): binary little-endian PLY, double coordinates
     def write_ply(self, path):
@@ -143,7 +194,8 @@ def extract_triangle_mesh(volume, with_colors: Optional[bool] = None) -> Triangl
         stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
         nb = volume.num_bricks()  # every brick ever opened = pool slots [0, nb)
         if nb == 0:
-            return TriangleMesh(np.zeros((0, 3)), np.zeros((0, 3), np.int64), np.zeros((0, 3)) if with_colors else None)
+            return TriangleMesh(np.zeros((0, 3)), np.zeros((0, 3), np.int64), np.zeros((0, 3)) if with_colors else None,
+                                device=dev)
         bricks = torch.arange(nb, dtype=torch.int32, device=dev)
         # edge keys are voxel indices inside the bounding box of the open bricks (+1: a cube reaches into its +1 neighbours)
         idx = volume._index[:nb, :3]
@@ -155,7 +207,8 @@ def extract_triangle_mesh(volume, with_colors: Optional[bool] = None) -> Triangl
         offsets = torch.cumsum(counts.to(torch.int64), 0) - counts.to(torch.int64)
         n_tri = int(counts.sum().item())
         if n_tri == 0:
-            return TriangleMesh(np.zeros((0, 3)), np.zeros((0, 3), np.int64), np.zeros((0, 3)) if with_colors else None)
+            return TriangleMesh(np.zeros((0, 3)), np.zeros((0, 3), np.int64), np.zeros((0, 3)) if with_colors else None,
+                                device=dev)
         keys = torch.empty(n_tri * 3, dtype=torch.int64, device=dev)
         _lib.check(L.gsb_mesh_emit(volume._h, window, ptr(bricks), nb, ptr(offsets.contiguous()), ptr(keys), stream))
         uniq, inverse = torch.unique(keys, return_inverse=True)  # vertex ids = rank of the edge key
@@ -164,7 +217,7 @@ def extract_triangle_mesh(volume, with_colors: Optional[bool] = None) -> Triangl
         rgb = torch.empty(nv, 3, dtype=torch.float64, device=dev) if with_colors else None
         _lib.check(L.gsb_mesh_vertices(volume._h, window, ptr(uniq.contiguous()), nv, ptr(xyz), ptr(rgb), stream))
         tris = inverse.reshape(-1, 3)
-        mesh = TriangleMesh(xyz.cpu().numpy(), tris.cpu().numpy(), None if rgb is None else rgb.cpu().numpy())
+        mesh = TriangleMesh(xyz.cpu().numpy(), tris.cpu().numpy(), None if rgb is None else rgb.cpu().numpy(), device=dev)
         mesh.edge_keys = uniq.cpu().numpy()  # (voxel index inside `key_window` * 3 + axis) per vertex, for tests
         mesh.key_window = (tuple(int(v) for v in lo), tuple(int(v) for v in (hi - lo + 2)))  # (brick origin, brick count)
     return mesh

@@ -105,7 +105,7 @@ class TriangleMesh(_Mesh):
 
     def __deepcopy__(self, memo):
         return TriangleMesh(self.vertices.copy(), self.triangles.copy(), None if self.vertex_colors is None else self.vertex_colors.copy(),
-                            None if self.vertex_normals is None else self.vertex_normals.copy())
+                            None if self.vertex_normals is None else self.vertex_normals.copy(), device=self.device)
 
 
 class ScalableTSDFVolume:
@@ -137,9 +137,7 @@ class ScalableTSDFVolume:
 
     def extract_triangle_mesh(self):
         m = _extract(self._vol)
-        out = TriangleMesh(m.vertices, m.triangles, m.vertex_colors, m.vertex_normals)
-        out._device = self._vol.device
-        return out
+        return TriangleMesh(m.vertices, m.triangles, m.vertex_colors, m.vertex_normals, device=m.device)
 
     def reset(self):
         self._vol.reset()

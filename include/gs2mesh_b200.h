@@ -325,6 +325,30 @@ int gsb_mesh_vertices(const GsbVolume* vol, const int32_t* window, const int64_t
 int gsb_mesh_vertex_normals(const double* xyz, int64_t n_vertices, const int64_t* triangles, int64_t n_triangles,
                             const int64_t* incidence, const int64_t* incidence_offsets, double* normals, void* stream);
 
+/* Cluster cleaning (gs2mesh_utils/tsdf_utils.py:122-142: TriangleMesh::ClusterConnectedTriangles, removal of the
+ * triangles of small clusters, remove_unreferenced_vertices).  triangles: device int64 [n_triangles,3], every index in
+ * [0, n_vertices) (not checked on the device).  n_triangles and n_vertices <= 2^31 - 1 (ids are 32-bit), otherwise
+ * GSB_ERR_INVALID.  Both entries use one caller workspace of gsb_mesh_cluster_workspace_bytes() (0 for invalid sizes).
+ *   gsb_mesh_clusters  triangles sharing an edge (either orientation; a degenerate edge (a,a) counts, a shared vertex
+ *                      does not) form a cluster.  labels[t]: device int64 [n_triangles], clusters numbered in the order
+ *                      of their smallest triangle (Open3D's and scipy's numbering); counts: device int64 [n_triangles],
+ *                      triangles per cluster in [0, *n_clusters); n_clusters: device int64.  cluster_area (device double
+ *                      [n_triangles], or NULL to skip; needs vertices = device double [n_vertices,3]): the sum of
+ *                      0.5*||(v1-v0) x (v2-v0)|| over each cluster, per triangle with numpy's roundings, summed in a
+ *                      fixed order (the same bits on every run, not numpy's sequential sum).
+ *   gsb_mesh_remove_small_clusters  given labels / counts of gsb_mesh_clusters: keeps triangle t iff
+ *                      !(counts[labels[t]] < threshold), in order, then the referenced vertices, in order.
+ *                      out_triangles: device int64 [n_triangles,3] (the kept triangles with new vertex ids);
+ *                      vertex_ids: device int64 [n_vertices] (old id of each kept vertex); sizes: device int64 [2] =
+ *                      (kept triangles, kept vertices). */
+size_t gsb_mesh_cluster_workspace_bytes(int64_t n_triangles, int64_t n_vertices);
+int gsb_mesh_clusters(const int64_t* triangles, int64_t n_triangles, int64_t n_vertices, const double* vertices, void* workspace,
+                      size_t workspace_bytes, int64_t* labels, int64_t* counts, int64_t* n_clusters, double* cluster_area,
+                      void* stream);
+int gsb_mesh_remove_small_clusters(const int64_t* triangles, int64_t n_triangles, int64_t n_vertices, const int64_t* labels,
+                                   const int64_t* counts, double threshold, void* workspace, size_t workspace_bytes,
+                                   int64_t* out_triangles, int64_t* vertex_ids, int64_t* sizes, void* stream);
+
 /* ------------------------------------------------------------------------------------------
  * Mesh-quality evaluation (evaluation/DTU/eval_code/eval.py, MobileBrick evaluate.py) without Open3D / sklearn.
  * All arithmetic is fp64 with explicit roundings (no FMA contraction), in the reference's operation order.
