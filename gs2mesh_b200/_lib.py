@@ -147,14 +147,37 @@ def lib() -> C.CDLL:
     return _lib
 
 
-def check(code: int) -> None:
+def check(code: int, invalid_is_value_error: bool = False) -> None:
+    """Raises GsbError for a failed call; with invalid_is_value_error, ValueError for GSB_ERR_INVALID instead (arguments
+    the caller passed on from its own caller)."""
     if code != GSB_OK:
-        raise GsbError(code, lib().gsb_last_error().decode("utf-8", "replace"))
+        message = lib().gsb_last_error().decode("utf-8", "replace")
+        if invalid_is_value_error and code == GSB_ERR_INVALID:
+            raise ValueError(message)
+        raise GsbError(code, message)
 
 
 def ptr(t):
     """torch tensor (or None) -> c_void_p of its storage start."""
     return None if t is None else C.c_void_p(t.data_ptr())
+
+
+def stream(dev) -> C.c_void_p:
+    """The current torch stream of CUDA device dev, as a library call's stream argument."""
+    import torch
+
+    return C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+
+
+def device(device=None, like=None):
+    """`device` if given, else the device of `like` when it is a CUDA tensor, else the current CUDA device."""
+    import torch
+
+    if device is not None:
+        return torch.device(device)
+    if isinstance(like, torch.Tensor) and like.is_cuda:
+        return like.device
+    return torch.device("cuda", torch.cuda.current_device())
 
 
 def profile_enable(on: bool) -> None:

@@ -121,6 +121,9 @@ struct StageTimer {
 
 inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
+// blocks of `threads` threads that cover n items
+inline unsigned blocks_for(long long n, int threads = 256) { return (unsigned)((n + threads - 1) / threads); }
+
 // ---------------------------------------------------------------------------------------------
 // Brick hash of the TSDF volume (Open3D's unordered_map<Vector3i, VolumeUnit>): open addressing, linear probing,
 // 64-bit keys = three 21-bit biased lattice indices.  An entry's position in the table identifies the brick inside a

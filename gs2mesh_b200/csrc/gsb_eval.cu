@@ -7,6 +7,7 @@
 
 #include "gs2mesh_b200.h"
 #include "gsb_common.h"
+#include "gsb_grid.cuh"
 
 namespace gsb {
 namespace {
@@ -24,9 +25,7 @@ struct Tri {
   double n1, n2;  // 0 when the triangle has zero area (eval.py:59-62 drops it)
 };
 
-__device__ __forceinline__ double norm3(const double* v) {
-  return __dsqrt_rn(__dadd_rn(__dadd_rn(__dmul_rn(v[0], v[0]), __dmul_rn(v[1], v[1])), __dmul_rn(v[2], v[2])));
-}
+__device__ __forceinline__ double norm3(const double* v) { return __dsqrt_rn(sq_norm3(v[0], v[1], v[2])); }
 
 __device__ Tri load_tri(const double* __restrict__ xyz, const long long* __restrict__ tris, long long t, double thresh) {
   Tri r;
@@ -114,13 +113,8 @@ __global__ void __launch_bounds__(256) sample_emit_kernel(const double* __restri
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
-// Uniform grid of reference points (counting sort of point ids by cell) and the exact 1-NN ring search over it.
+// Uniform grid of reference points (gsb_grid.cuh): counting sort of point ids by cell, exact 1-NN ring search over it.
 // ---------------------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ int cell_axis(double p, double o, double h, int dim) {
-  const double c = floor((p - o) / h);
-  return c < 0.0 ? 0 : (c >= (double)dim ? dim - 1 : (int)c);
-}
-
 __global__ void __launch_bounds__(256) grid_count_kernel(const GsbPointGrid g, int* __restrict__ cell_of,
                                                          unsigned long long* __restrict__ counts) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -153,12 +147,11 @@ __global__ void __launch_bounds__(256) grid_scatter_kernel(const GsbPointGrid g,
 // The ring bound's relative margin kRingMargin must exceed the rounding error of the cell indices.  A query's or a
 // point's index (p - o) / h rounds twice, so it is off by at most 2^-52 * |index| cells.  A point in ring k of a query
 // has |index| < dims and the query |index| <= k + dims, so the two are off by at most 2^-52 * (k + 2*dims) cells, which
-// stays below kRingMargin * (k - 1) for every k >= 2 while dims <= kMaxAxisCells (9.3e-10 at k = 2; grid_ok refuses
-// larger axes).  The distance expression's own rounding (a few ulp) is far below the margin.  PointGrid's cell floor of
-// (hi - lo) / 1e6 keeps every axis at about 1e6 cells: a change to that floor must keep it within kMaxAxisCells.
+// stays below kRingMargin * (k - 1) for every k >= 2 while dims <= kMaxAxisCells (9.3e-10 at k = 2; gsb_grid.cuh's
+// grid_ok refuses larger axes).  The distance expression's own rounding (a few ulp) is far below the margin.  PointGrid's
+// cell floor of (hi - lo) / 1e6 keeps every axis at about 1e6 cells: a change to that floor must keep it within the limit.
 constexpr double kFarCells = 1099511627776.0;  // 2^40
 constexpr double kRingMargin = 1e-9;
-constexpr int kMaxAxisCells = 1 << 21;
 
 struct Nearest {
   double d2;
@@ -202,9 +195,7 @@ __device__ __forceinline__ Nearest ring_nearest(const GsbPointGrid& g, double qx
           const long long c = (x * g.dims[1] + y) * g.dims[2] + zz;
           for (long long s = g.cell_start[c], e = g.cell_start[c + 1]; s < e; ++s) {
             const long long id = g.ids[s];
-            const double* p = g.points + 3 * id;
-            const double dx = __dsub_rn(qx, p[0]), dy = __dsub_rn(qy, p[1]), dz = __dsub_rn(qz, p[2]);
-            const double d2 = __dadd_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)), __dmul_rn(dz, dz));
+            const double d2 = sq_dist(qx, qy, qz, g.points + 3 * id);
             if (d2 < best2 || (d2 == best2 && id < best)) {
               best2 = d2;
               best = id;
@@ -254,29 +245,19 @@ __global__ void __launch_bounds__(128) downsample_round_kernel(const GsbPointGri
                                                                unsigned int* __restrict__ undecided) {
   const long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (p >= g.n_points || state[p] != 0) return;
-  const double px = g.points[3 * p], py = g.points[3 * p + 1], pz = g.points[3 * p + 2];
-  const int cx = cell_axis(px, g.origin[0], g.cell, g.dims[0]), cy = cell_axis(py, g.origin[1], g.cell, g.dims[1]),
-            cz = cell_axis(pz, g.origin[2], g.cell, g.dims[2]);
   const double* __restrict__ pts = g.points;
-  const int64_t* __restrict__ start = g.cell_start;
-  const int64_t* __restrict__ ids = g.ids;
+  const double px = pts[3 * p], py = pts[3 * p + 1], pz = pts[3 * p + 2];
   bool pending = false;
-  for (int nb = 0; nb < 27; ++nb) {
-    const int x = cx + nb / 9 - 1, y = cy + (nb / 3) % 3 - 1, z = cz + nb % 3 - 1;
-    if (x < 0 || x >= g.dims[0] || y < 0 || y >= g.dims[1] || z < 0 || z >= g.dims[2]) continue;
-    const long long c = ((long long)x * g.dims[1] + y) * g.dims[2] + z;
-    for (long long s = start[c], e = start[c + 1]; s < e; ++s) {
-      const long long q = ids[s];
-      if (q >= p) continue;
-      const double dx = __dsub_rn(px, pts[3 * q]), dy = __dsub_rn(py, pts[3 * q + 1]), dz = __dsub_rn(pz, pts[3 * q + 2]);
-      if (!(__dadd_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)), __dmul_rn(dz, dz)) <= r2)) continue;
-      const unsigned char sq = *((volatile unsigned char*)state + q);
-      if (sq == 1) {
-        state[p] = 2;
-        return;
-      }
-      if (sq == 0) pending = true;
-    }
+  const bool dropped = !visit_27_cells(g, px, py, pz, [&](long long q) {
+    if (q >= p || !(sq_dist(px, py, pz, pts + 3 * q) <= r2)) return true;
+    const unsigned char sq = *((volatile unsigned char*)state + q);
+    if (sq == 1) return false;  // a kept earlier neighbour: p is dropped
+    if (sq == 0) pending = true;
+    return true;
+  });
+  if (dropped) {
+    state[p] = 2;
+    return;
   }
   if (!pending) {
     state[p] = 1;
@@ -288,16 +269,6 @@ __global__ void __launch_bounds__(128) downsample_round_kernel(const GsbPointGri
 __global__ void __launch_bounds__(256) downsample_finish_kernel(unsigned char* __restrict__ state, long long n) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) state[i] = state[i] == 1;
-}
-
-bool grid_ok(const GsbPointGrid* g) {
-  if (!g || g->n_points < 0 || (g->n_points && !g->points) || !g->cell_start || !(g->cell > 0.0)) return false;
-  double cells = 1.0;
-  for (int a = 0; a < 3; ++a) {
-    if (g->dims[a] <= 0 || g->dims[a] > kMaxAxisCells) return false;  // the ring bound's margin covers kMaxAxisCells
-    cells *= g->dims[a];
-  }
-  return cells < 2147483647.0;
 }
 
 long long grid_cells(const GsbPointGrid* g) { return (long long)g->dims[0] * g->dims[1] * g->dims[2]; }
@@ -352,7 +323,7 @@ size_t gsb_eval_grid_workspace_bytes(int64_t n_points, int64_t n_cells) {
 
 int gsb_eval_grid_build(const GsbPointGrid* grid, void* workspace, size_t workspace_bytes, void* stream_v) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
-  if (!grid_ok(grid) || (grid->n_points && !grid->ids) || !workspace) return fail(GSB_ERR_INVALID, "eval_grid_build: bad arguments");
+  if (!grid_ok(grid) || !workspace) return fail(GSB_ERR_INVALID, "eval_grid_build: bad arguments");
   const long long cells = grid_cells(grid), n = grid->n_points;
   if (workspace_bytes < gsb_eval_grid_workspace_bytes(n, cells))
     return fail(GSB_ERR_WORKSPACE, "eval_grid_build: workspace %zu < %zu bytes", workspace_bytes,
@@ -378,8 +349,7 @@ int gsb_eval_grid_build(const GsbPointGrid* grid, void* workspace, size_t worksp
 int gsb_eval_nearest(const GsbPointGrid* grid, const double* queries, int64_t n_queries, double max_dist, double* dist,
                      int64_t* index, void* stream_v) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
-  if (!grid_ok(grid) || (grid->n_points && !grid->ids) || n_queries < 0 || (n_queries && (!queries || !dist || !index)) ||
-      !(max_dist > 0.0))
+  if (!grid_ok(grid) || n_queries < 0 || (n_queries && (!queries || !dist || !index)) || !(max_dist > 0.0))
     return fail(GSB_ERR_INVALID, "eval_nearest: bad arguments");
   if (n_queries == 0) return GSB_OK;
   nearest_kernel<<<(unsigned)((n_queries + 127) / 128), 128, 0, stream>>>(*grid, queries, n_queries, max_dist, dist,
@@ -391,8 +361,8 @@ int gsb_eval_nearest(const GsbPointGrid* grid, const double* queries, int64_t n_
 int gsb_eval_icp_correspond(const GsbPointGrid* grid, const double* source, int64_t n_source, double radius, int64_t* index,
                             double* dist2, void* stream_v) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
-  if (!grid_ok(grid) || (grid->n_points && !grid->ids) || n_source < 0 || (n_source && (!source || !index || !dist2)) ||
-      !(radius > 0.0) || !(radius < INFINITY))
+  if (!grid_ok(grid) || n_source < 0 || (n_source && (!source || !index || !dist2)) || !(radius > 0.0) ||
+      !(radius < INFINITY))
     return fail(GSB_ERR_INVALID, "eval_icp_correspond: bad arguments");
   if (n_source == 0) return GSB_OK;
   icp_correspond_kernel<<<(unsigned)((n_source + 127) / 128), 128, 0, stream>>>(*grid, source, n_source, radius, radius * radius,
@@ -404,7 +374,7 @@ int gsb_eval_icp_correspond(const GsbPointGrid* grid, const double* source, int6
 int gsb_eval_radius_downsample(const GsbPointGrid* grid, double radius, uint8_t* keep, uint32_t* counters,
                                uint32_t* host_undecided, int32_t* rounds, void* stream_v) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
-  if (!grid_ok(grid) || (grid->n_points && (!grid->ids || !keep || !counters || !host_undecided)) || !(radius >= 0.0) ||
+  if (!grid_ok(grid) || (grid->n_points && (!keep || !counters || !host_undecided)) || !(radius >= 0.0) ||
       !(grid->cell >= radius * 1.0000001))
     return fail(GSB_ERR_INVALID, "eval_radius_downsample: bad arguments (the grid cell must exceed the radius)");
   const long long n = grid->n_points;

@@ -406,8 +406,6 @@ __global__ void clean_sizes_kernel(const int* __restrict__ keep, const int* __re
   sizes[1] = nv ? (long long)new_id[nv - 1] + referenced[nv - 1] : 0;
 }
 
-inline unsigned blocks_of(long long n, int per_block = 256) { return (unsigned)((n + per_block - 1) / per_block); }
-
 inline int bits_of(unsigned long long max_value) {
   int b = 0;
   while (b < 64 && (max_value >> b) != 0) ++b;
@@ -571,17 +569,17 @@ int gsb_mesh_clusters(const int64_t* triangles, int64_t n_triangles, int64_t n_v
   const unsigned long long stride = (unsigned long long)n_vertices + 1;
   const int key_bits = bits_of(stride * stride - 1);  // keys < (n_vertices+1)^2
 
-  cluster_edge_keys_kernel<<<blocks_of(nt), 256, 0, stream>>>(tris, nt, stride, w.keys, w.owner, w.parent);
+  cluster_edge_keys_kernel<<<blocks_for(nt), 256, 0, stream>>>(tris, nt, stride, w.keys, w.owner, w.parent);
   count_launch();
   cub::DoubleBuffer<unsigned long long> keys(w.keys, w.keys + n3);
   cub::DoubleBuffer<uint32_t> owner(w.owner, w.owner + n3);
   size_t tmp_bytes = w.tmp_bytes;
   GSB_CUDA_OK(cub::DeviceRadixSort::SortPairs(w.tmp, tmp_bytes, keys, owner, n3, 0, key_bits, stream));
   if (n3 > 1) {
-    cluster_union_kernel<<<blocks_of(n3 - 1), 256, 0, stream>>>(keys.Current(), owner.Current(), n3, w.parent);
+    cluster_union_kernel<<<blocks_for(n3 - 1), 256, 0, stream>>>(keys.Current(), owner.Current(), n3, w.parent);
     count_launch();
   }
-  cluster_compress_kernel<<<blocks_of(nt), 256, 0, stream>>>(w.parent, nt, w.flag);
+  cluster_compress_kernel<<<blocks_for(nt), 256, 0, stream>>>(w.parent, nt, w.flag);
   count_launch();
   tmp_bytes = w.tmp_bytes;
   GSB_CUDA_OK(cub::DeviceScan::ExclusiveSum(w.tmp, tmp_bytes, w.flag, w.rank, (long long)nt, stream));
@@ -589,7 +587,7 @@ int gsb_mesh_clusters(const int64_t* triangles, int64_t n_triangles, int64_t n_v
   GSB_CUDA_OK(cudaMemsetAsync(counts, 0, sizeof(int64_t) * (size_t)nt, stream));
   // the edge sort's buffers are free from here on: labels as sort keys in `owner`, areas and offsets in `keys`
   uint32_t* label32 = cluster_area ? w.owner : nullptr;
-  cluster_label_kernel<<<blocks_of(nt), 256, 0, stream>>>(w.parent, w.flag, w.rank, nt, reinterpret_cast<long long*>(labels),
+  cluster_label_kernel<<<blocks_for(nt), 256, 0, stream>>>(w.parent, w.flag, w.rank, nt, reinterpret_cast<long long*>(labels),
                                                           ucounts, reinterpret_cast<long long*>(n_clusters), label32);
   count_launch();
   if (int rc = check_launch("mesh_clusters", stream, false)) return rc;
@@ -597,7 +595,7 @@ int gsb_mesh_clusters(const int64_t* triangles, int64_t n_triangles, int64_t n_v
 
   auto* area = reinterpret_cast<double*>(w.keys);
   auto* offsets = reinterpret_cast<long long*>(w.keys + 2 * (size_t)nt);
-  triangle_area_kernel<<<blocks_of(nt), 256, 0, stream>>>(vertices, tris, nt, area);
+  triangle_area_kernel<<<blocks_for(nt), 256, 0, stream>>>(vertices, tris, nt, area);
   count_launch();
   cub::DoubleBuffer<uint32_t> by_label(label32, label32 + nt);
   cub::DoubleBuffer<double> areas(area, area + nt);
@@ -606,7 +604,7 @@ int gsb_mesh_clusters(const int64_t* triangles, int64_t n_triangles, int64_t n_v
                                               stream));
   tmp_bytes = w.tmp_bytes;
   GSB_CUDA_OK(cub::DeviceScan::ExclusiveSum(w.tmp, tmp_bytes, ucounts, offsets, (long long)nt, stream));
-  cluster_area_sum_kernel<<<blocks_of(32 * (long long)nt), 256, 0, stream>>>(areas.Current(), offsets, ucounts, nt, cluster_area);
+  cluster_area_sum_kernel<<<blocks_for(32 * (long long)nt), 256, 0, stream>>>(areas.Current(), offsets, ucounts, nt, cluster_area);
   count_launch();
   return check_launch("mesh_clusters(area)", stream, false);
 }
@@ -627,7 +625,7 @@ int gsb_mesh_remove_small_clusters(const int64_t* triangles, int64_t n_triangles
   const auto* tris = reinterpret_cast<const long long*>(triangles);
   size_t tmp_bytes;
   if (nt) {
-    cluster_keep_kernel<<<blocks_of(nt), 256, 0, stream>>>(reinterpret_cast<const long long*>(labels),
+    cluster_keep_kernel<<<blocks_for(nt), 256, 0, stream>>>(reinterpret_cast<const long long*>(labels),
                                                            reinterpret_cast<const long long*>(counts), nt, threshold, w.keep);
     count_launch();
     tmp_bytes = w.tmp_bytes;
@@ -636,16 +634,16 @@ int gsb_mesh_remove_small_clusters(const int64_t* triangles, int64_t n_triangles
   if (nv) {
     GSB_CUDA_OK(cudaMemsetAsync(w.referenced, 0, sizeof(int) * (size_t)nv, stream));
     if (nt) {
-      mark_referenced_kernel<<<blocks_of(nt), 256, 0, stream>>>(tris, w.keep, nt, w.referenced);
+      mark_referenced_kernel<<<blocks_for(nt), 256, 0, stream>>>(tris, w.keep, nt, w.referenced);
       count_launch();
     }
     tmp_bytes = w.tmp_bytes;
     GSB_CUDA_OK(cub::DeviceScan::ExclusiveSum(w.tmp, tmp_bytes, w.referenced, w.new_id, (long long)nv, stream));
-    kept_vertices_kernel<<<blocks_of(nv), 256, 0, stream>>>(w.referenced, w.new_id, nv, reinterpret_cast<long long*>(vertex_ids));
+    kept_vertices_kernel<<<blocks_for(nv), 256, 0, stream>>>(w.referenced, w.new_id, nv, reinterpret_cast<long long*>(vertex_ids));
     count_launch();
   }
   if (nt) {
-    remap_triangles_kernel<<<blocks_of(nt), 256, 0, stream>>>(tris, w.keep, w.tri_pos, w.new_id, nt,
+    remap_triangles_kernel<<<blocks_for(nt), 256, 0, stream>>>(tris, w.keep, w.tri_pos, w.new_id, nt,
                                                               reinterpret_cast<long long*>(out_triangles));
     count_launch();
   }

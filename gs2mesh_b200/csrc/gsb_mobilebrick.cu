@@ -7,13 +7,10 @@
 // an add into an FMA.
 #include "gs2mesh_b200.h"
 #include "gsb_common.h"
+#include "gsb_grid.cuh"
 
 namespace gsb {
 namespace {
-
-__device__ __forceinline__ double sq_norm3(double x, double y, double z) {
-  return __dadd_rn(__dadd_rn(__dmul_rn(x, x), __dmul_rn(y, y)), __dmul_rn(z, z));
-}
 
 // GetSurfaceArea's per-triangle term: 0.5 * ((p0 - p1).cross(p0 - p2)).norm()
 __global__ void __launch_bounds__(256) triangle_area_kernel(const double* __restrict__ v, const long long* __restrict__ tris,
@@ -69,11 +66,6 @@ __global__ void __launch_bounds__(256) sample_uniform_kernel(const double* __res
 // Poisson-disk elimination.  Neighbours of p: every q != p with ((dx*dx)+dy*dy)+dz*dz < r_max^2 (nanoflann's radius
 // search, strict), dx = p.x - q.x.  The grid's cell is >= r_max, so they lie in the 27 cells around p's cell.
 // ---------------------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ int cell_of(double p, double o, double h, int dim) {
-  const double c = floor((p - o) / h);
-  return c < 0.0 ? 0 : (c >= (double)dim ? dim - 1 : (int)c);
-}
-
 template <bool kEmit>
 __global__ void __launch_bounds__(128) neighbour_kernel(const GsbPointGrid g, double r2, long long* __restrict__ counts,
                                                         const long long* __restrict__ offsets, int* __restrict__ nbr,
@@ -81,36 +73,28 @@ __global__ void __launch_bounds__(128) neighbour_kernel(const GsbPointGrid g, do
   const long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (p >= g.n_points) return;
   const double px = g.points[3 * p], py = g.points[3 * p + 1], pz = g.points[3 * p + 2];
-  const int cx = cell_of(px, g.origin[0], g.cell, g.dims[0]), cy = cell_of(py, g.origin[1], g.cell, g.dims[1]),
-            cz = cell_of(pz, g.origin[2], g.cell, g.dims[2]);
   long long n = 0;
   const long long base = kEmit ? offsets[p] : 0;
-  for (int c27 = 0; c27 < 27; ++c27) {
-    const int x = cx + c27 / 9 - 1, y = cy + (c27 / 3) % 3 - 1, z = cz + c27 % 3 - 1;
-    if (x < 0 || x >= g.dims[0] || y < 0 || y >= g.dims[1] || z < 0 || z >= g.dims[2]) continue;
-    const long long c = ((long long)x * g.dims[1] + y) * g.dims[2] + z;
-    for (long long s = g.cell_start[c], e = g.cell_start[c + 1]; s < e; ++s) {
-      const long long q = g.ids[s];
-      if (q == p) continue;
-      const double d2 = sq_norm3(__dsub_rn(px, g.points[3 * q]), __dsub_rn(py, g.points[3 * q + 1]),
-                                 __dsub_rn(pz, g.points[3 * q + 2]));
-      if (!(d2 < r2)) continue;
-      if (kEmit) {  // insertion into the (d2, q)-sorted list of this point's slice
-        long long k = n;
-        while (k > 0) {
-          const double dk = d2_out[base + k - 1];
-          const int qk = nbr[base + k - 1];
-          if (dk < d2 || (dk == d2 && qk < q)) break;
-          d2_out[base + k] = dk;
-          nbr[base + k] = qk;
-          --k;
-        }
-        d2_out[base + k] = d2;
-        nbr[base + k] = (int)q;
+  visit_27_cells(g, px, py, pz, [&](long long q) {
+    if (q == p) return true;
+    const double d2 = sq_dist(px, py, pz, g.points + 3 * q);
+    if (!(d2 < r2)) return true;
+    if (kEmit) {  // insertion into the (d2, q)-sorted list of this point's slice
+      long long k = n;
+      while (k > 0) {
+        const double dk = d2_out[base + k - 1];
+        const int qk = nbr[base + k - 1];
+        if (dk < d2 || (dk == d2 && qk < q)) break;
+        d2_out[base + k] = dk;
+        nbr[base + k] = qk;
+        --k;
       }
-      ++n;
+      d2_out[base + k] = d2;
+      nbr[base + k] = (int)q;
     }
-  }
+    ++n;
+    return true;
+  });
   if (!kEmit) counts[p] = n;
 }
 
@@ -181,18 +165,6 @@ __global__ void __launch_bounds__(256) visibility_kernel(const double* __restric
   keep[i] = inside && volume[((long long)idx[0] * r1 + idx[1]) * r2 + idx[2]] != 0;
 }
 
-bool grid_ok(const GsbPointGrid* g) {
-  if (!g || g->n_points < 0 || g->n_points >= 2147483647 || (g->n_points && (!g->points || !g->ids)) || !g->cell_start ||
-      !(g->cell > 0.0))
-    return false;
-  double cells = 1.0;
-  for (int a = 0; a < 3; ++a) {
-    if (g->dims[a] <= 0) return false;
-    cells *= g->dims[a];
-  }
-  return cells < 2147483647.0;
-}
-
 }  // namespace
 }  // namespace gsb
 
@@ -231,8 +203,9 @@ int gsb_eval_poisson_neighbours(const GsbPointGrid* grid, double r_max, double r
                                 const int64_t* offsets, int32_t* neighbours, double* terms, void* stream_v) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
   const bool emit = offsets != nullptr;
-  if (!grid_ok(grid) || !(r_max > 0.0) || !(r_max < INFINITY) || !(r_min >= 0.0) || !(r_min <= r_max) ||
-      !(grid->cell >= r_max * 1.0000001) || (grid->n_points && (emit ? (!neighbours || !terms) : !counts)))
+  if (!grid_ok(grid) || grid->n_points >= 2147483647 ||  // the neighbour ids are int32
+      !(r_max > 0.0) || !(r_max < INFINITY) || !(r_min >= 0.0) || !(r_min <= r_max) || !(grid->cell >= r_max * 1.0000001) ||
+      (grid->n_points && (emit ? (!neighbours || !terms) : !counts)))
     return fail(GSB_ERR_INVALID,
                 "eval_poisson_neighbours: bad arguments (0 <= r_min <= r_max finite, the grid cell must exceed r_max, "
                 "fewer than 2^31 points)");

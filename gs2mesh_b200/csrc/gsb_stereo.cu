@@ -27,8 +27,6 @@ bool frame_ok(int width, int height) {
   return width >= 1 && height >= 1 && width <= GSB_TSDF_MAX_WIDTH && height <= GSB_TSDF_MAX_HEIGHT;
 }
 
-unsigned blocks_for(long long n) { return (unsigned)((n + 255) / 256); }
-
 // One thread per padded pixel of each of the 4 images: [0] = pad(left), [1] = pad(right), [2] = flip_x(pad(right)),
 // [3] = flip_x(pad(left)); replicate padding, float(u8), channel planes [4][3][Hp][Wp].
 __global__ void __launch_bounds__(256) pack_kernel(const uint8_t* __restrict__ left, const uint8_t* __restrict__ right, int width,

@@ -203,8 +203,6 @@ __global__ void __launch_bounds__(kMomThreads) moments_final_kernel(const double
   if (lane == 0) out[kMomSums] = (double)sc[0];
 }
 
-unsigned blocks_for(long long n) { return (unsigned)((n + 255) / 256); }
-
 int bits_for(long long extent) {  // bits that hold 0 .. extent - 1
   int b = 0;
   while (b < 63 && (1ll << b) < extent) ++b;

@@ -18,7 +18,6 @@ coordinates, which trimesh would drop on load.
 from __future__ import annotations
 
 import argparse
-import ctypes as C
 import glob
 import os
 
@@ -30,19 +29,6 @@ from ._lib import ptr
 
 IMAGE_SIZE = (1600, 1200)  # W, H of evaluate_single_scene.py:47: the frame pixel coordinates are normalised to
 RADIUS = 24  # disk(24), evaluate_single_scene.py:80
-
-
-def _device(device, x=None):
-    """`device` if given, else the device of a CUDA tensor x, else the current CUDA device."""
-    if device is not None:
-        return torch.device(device)
-    if isinstance(x, torch.Tensor) and x.is_cuda:
-        return x.device
-    return torch.device("cuda", torch.cuda.current_device())
-
-
-def _stream(dev):
-    return C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
 
 
 def _mask_stack(masks):
@@ -67,14 +53,14 @@ def _dilate_packed(masks, radius):
     work = torch.empty(V * H * W, dtype=torch.uint8, device=dev)
     with torch.cuda.device(dev):
         _lib.check(_lib.lib().gsb_eval_mask_dilate_disk(ptr(masks), V, H, W, int(radius), ptr(packed), ptr(work),
-                                                        _stream(dev)))
+                                                        _lib.stream(dev)))
     return packed
 
 
 def dilate_masks(masks, radius=RADIUS, device=None):
     """Each mask's set (nonzero) pixels dilated by skimage's disk(radius), x*x + y*y <= radius*radius, with pixels
     outside the image unset -> device bool [V,H,W]."""
-    m = _mask_stack(masks).to(_device(device, masks)).contiguous()
+    m = _mask_stack(masks).to(_lib.device(device, masks)).contiguous()
     V, H, W = m.shape
     packed = _dilate_packed(m, radius)
     bits = torch.arange(32, dtype=torch.int32, device=m.device)
@@ -95,7 +81,7 @@ def cull_vertices(vertices, matrices, masks, image_size=IMAGE_SIZE, radius=RADIU
     if len(masks) < n_views:
         raise ValueError(f"cull_vertices: {len(masks)} masks for {n_views} views")
     m = _mask_stack(masks[:n_views])
-    dev = _device(device, vertices)
+    dev = _lib.device(device, vertices)
     v, M, m = v.to(dev).contiguous(), M.to(dev).contiguous(), m.to(dev).contiguous()
     W, H = (int(s) for s in image_size)
     n = v.shape[0]
@@ -104,7 +90,7 @@ def cull_vertices(vertices, matrices, masks, image_size=IMAGE_SIZE, radius=RADIU
         packed = _dilate_packed(m, radius)
         with torch.cuda.device(dev):
             _lib.check(_lib.lib().gsb_eval_cull_vertices_by_masks(ptr(v), n, ptr(M), n_views, W, H, m.shape[2], m.shape[1],
-                                                                  ptr(packed), ptr(keep), _stream(dev)))
+                                                                  ptr(packed), ptr(keep), _lib.stream(dev)))
     return keep.bool()
 
 
@@ -112,17 +98,13 @@ def cull_mesh(vertices, triangles, matrices, masks, scale_mat, image_size=IMAGE_
     """evaluate_single_scene.py:57-114: the kept vertices in order, moved to DTU world coordinates with
     v * scale_mat[0,0] + scale_mat[:3,3] (float64), and the faces whose three vertices are kept, in order, remapped.
     Returns a TriangleMesh."""
-    from .mesh import TriangleMesh
+    from .mesh import TriangleMesh, remove_vertices_by_mask
 
     keep = cull_vertices(vertices, matrices, masks, image_size, radius, device)
-    dev = keep.device
-    v = torch.as_tensor(vertices).to(dev).to(torch.float64).reshape(-1, 3)
-    t = torch.as_tensor(np.asarray(triangles, np.int64)).to(dev).reshape(-1, 3)
-    face_keep = keep[t].all(dim=1)
-    remap = torch.cumsum(keep.to(torch.int64), 0) - 1
+    v, t, _, _ = remove_vertices_by_mask(torch.as_tensor(vertices).to(keep.device), np.asarray(triangles, np.int64), ~keep)
     s = np.asarray(scale_mat, np.float32)
-    world = v[keep] * float(s[0, 0]) + torch.as_tensor(s[:3, 3].astype(np.float64), device=dev)
-    return TriangleMesh(world.cpu().numpy(), remap[t[face_keep]].cpu().numpy())
+    world = v * float(s[0, 0]) + torch.as_tensor(s[:3, 3].astype(np.float64), device=v.device)
+    return TriangleMesh(world.cpu().numpy(), t.cpu().numpy())
 
 
 def decompose_projection(P):
@@ -143,7 +125,7 @@ def dtu_cameras(instance_dir, device=None):
     """evaluate_single_scene.py:24-38, 64-66 with the same library calls on the same dtypes: the projection matrices
     intrinsic.float() @ inverse(pose) (float32 [V,4,4] on the device, the inverse taken on the CPU) and scale_mat_i
     (float32 numpy) of the first V = len(images/*.png) views."""
-    dev = _device(device)
+    dev = _lib.device(device)
     n_images = len(glob.glob(os.path.join(instance_dir, "images", "*.png")))
     camera_dict = np.load(os.path.join(instance_dir, "cameras.npz"))
     scale_mats = [camera_dict["scale_mat_%d" % i].astype(np.float32) for i in range(n_images)]

@@ -23,11 +23,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from ._lib import ptr
-
-
-def _stream(dev):
-    return C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+from ._lib import ptr, stream as _stream
 
 
 def _points(x, dev=None):
@@ -67,9 +63,9 @@ def grid_layout(lo, hi, core, n, cells_per_point=4.0, min_cell=0.0, max_cells=1 
     """(cell, dims) of PointGrid for n points with bounds lo / hi and 1%..99% quantile extent `core` per axis.
 
     The cell never falls below (hi - lo).max() * 1e-6, so no axis has more than about 1e6 cells: the ring search's
-    rounding margin (gsb_eval.cu, kRingMargin) covers up to 2^21.  When the points coincide (an extent of 1e-294 or less)
-    the cell is tied to the coordinates' magnitude instead, max(|lo|, |hi|, 1) * 2^-30: one cell holds them all, and the
-    cell stays a normal number, so the search's distance bounds keep their precision."""
+    rounding margin (gsb_eval.cu, kRingMargin) covers up to 2^21 (gsb_grid.cuh, kMaxAxisCells).  When the points coincide
+    (an extent of 1e-294 or less) the cell is tied to the coordinates' magnitude instead, max(|lo|, |hi|, 1) * 2^-30: one
+    cell holds them all, and the cell stays a normal number, so the search's distance bounds keep their precision."""
     lo, hi, core = (np.asarray(x, dtype=np.float64) for x in (lo, hi, core))
     big = float(core.max())
     cell = (float(np.prod(np.maximum(core, big * 1e-3))) / (cells_per_point * n)) ** (1.0 / 3.0) if big > 0 else 0.0
@@ -88,10 +84,12 @@ class PointGrid:
     """Reference points bucketed into a uniform grid (gsb_eval_grid_build), reusable for many nearest() queries.
 
     The cell size comes from the point spacing inside the 1%..99% quantile box of each axis (so a few far floaters do not
-    stretch the cells over the whole object), never below min_cell; the grid then covers every point, and the cell grows
-    only when that would need more than max_cells cells (grid_layout)."""
+    stretch the cells over the whole object), never below min_cell nor radius * 1.001; the grid then covers every point,
+    and the cell grows only when that would need more than max_cells cells (grid_layout).  radius is the largest search
+    radius of the 27-cell searches (gsb_eval_radius_downsample, gsb_eval_poisson_neighbours), which refuse a cell below
+    radius * 1.0000001."""
 
-    def __init__(self, reference, cells_per_point=4.0, min_cell=0.0, max_cells=1 << 26):
+    def __init__(self, reference, radius=0.0, cells_per_point=4.0, min_cell=0.0, max_cells=1 << 26):
         self.points = _points(reference)
         dev = self.points.device
         n = self.points.shape[0]
@@ -105,7 +103,8 @@ class PointGrid:
         srt = sub.sort(dim=0).values
         m = srt.shape[0]
         core = (srt[min(m - 1, int(0.99 * m))] - srt[int(0.01 * m)]).cpu().numpy()
-        cell, dims = grid_layout(lo, hi, core, n, cells_per_point, min_cell, max_cells)
+        cell, dims = grid_layout(lo, hi, core, n, cells_per_point, max(float(min_cell), float(radius) * 1.001),
+                                 max_cells)
         self.origin, self.cell, self.dims = lo, cell, dims
         cells = dims[0] * dims[1] * dims[2]
         self.cell_start = torch.empty(cells + 1, dtype=torch.int64, device=dev)
@@ -169,7 +168,7 @@ def radius_downsample(points, radius, seed=0, order=None):
     shuffled = p[order].contiguous()
     keep = torch.zeros(n, dtype=torch.uint8, device=dev)
     if n:
-        grid = PointGrid(shuffled, min_cell=float(radius) * 1.001)
+        grid = PointGrid(shuffled, radius)
         counters = torch.empty(4, dtype=torch.int32, device=dev)
         host = torch.empty(1, dtype=torch.int32).pin_memory()
         with torch.cuda.device(dev):
@@ -184,7 +183,7 @@ def dtu_chamfer(data, stl_points, obs_mask, bb, res, plane, *, mode="mesh", down
     reference scan; obs_mask / bb / res the ObsMask .mat fields, plane its Plane .mat field P.  Returns mean_d2s,
     mean_s2d, overall (numpy float64, bit-identical to eval.py run with np.random.default_rng(seed)) and the per-point
     arrays the visualisation needs."""
-    dev = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
+    dev = _lib.device(device)
     thresh = downsample_density
     if mode == "mesh":
         vertices, triangles = data

@@ -58,7 +58,7 @@ class TriangleMesh:
             return self
         if nt and (self.triangles.min() < 0 or self.triangles.max() >= nv):
             raise ValueError("compute_vertex_normals: triangle vertex index out of range")
-        dev = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
+        dev = _lib.device(device)
         with torch.cuda.device(dev):
             xyz = torch.as_tensor(self.vertices).to(dev).contiguous()
             tri = torch.as_tensor(self.triangles).to(dev).contiguous()
@@ -69,7 +69,7 @@ class TriangleMesh:
             offsets = torch.zeros(nv + 1, dtype=torch.int64, device=dev)
             offsets[1:] = torch.cumsum(torch.bincount(flat, minlength=nv), 0)
             out = torch.empty(nv, 3, dtype=torch.float64, device=dev)
-            stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+            stream = _lib.stream(dev)
             _lib.check(_lib.lib().gsb_mesh_vertex_normals(ptr(xyz), nv, ptr(tri), nt, ptr(incidence), ptr(offsets), ptr(out),
                                                           stream))
             self.vertex_normals = out.cpu().numpy()
@@ -83,7 +83,7 @@ class TriangleMesh:
             raise ValueError("cluster_connected_triangles: triangle vertex index out of range")
         dev = self.device
         L = _lib.lib()
-        stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+        stream = _lib.stream(dev)
         tri = torch.as_tensor(self.triangles, dtype=torch.int64).to(dev).contiguous()
         work = torch.empty(L.gsb_mesh_cluster_workspace_bytes(nt, nv), dtype=torch.uint8, device=dev)
         labels = torch.empty(nt, dtype=torch.int64, device=dev)
@@ -143,7 +143,7 @@ class TriangleMesh:
         nv, nt = len(self.vertices), len(self.triangles)
         with torch.cuda.device(self.device):
             dev = self.device
-            stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+            stream = _lib.stream(dev)
             tri, work, labels, counts, _, _ = self._clusters_on_device(with_area=False)
             out_tri = torch.empty(nt, 3, dtype=torch.int64, device=dev)
             ids = torch.empty(nv, dtype=torch.int64, device=dev)
@@ -185,13 +185,32 @@ class TriangleMesh:
         return path
 
 
+def remove_vertices_by_mask(vertices, triangles, vertex_mask, vertex_colors=None, vertex_normals=None):
+    """TriangleMesh.remove_vertices_by_mask(mask): drops the vertices where vertex_mask is True, keeping the rest (and
+    their colours and normals) in order; keeps the triangles whose three vertices survive, in order, re-indexed.
+    Vertices no triangle uses stay.  Returns (vertices, triangles, colours or None, normals or None) as device tensors."""
+    v = torch.as_tensor(vertices)
+    dev = _lib.device(like=v)
+    v = v.to(dev).to(torch.float64).reshape(-1, 3)
+    t = torch.as_tensor(triangles).to(dev).to(torch.int64).reshape(-1, 3)
+    keep = ~torch.as_tensor(vertex_mask).to(dev).to(torch.bool).reshape(-1)
+    if keep.shape[0] != v.shape[0]:
+        raise ValueError("remove_vertices_by_mask: the mask must have one entry per vertex")
+    vmap = torch.cumsum(keep.to(torch.int64), 0) - 1
+    vmap = torch.where(keep, vmap, torch.full_like(vmap, -1))
+    mt = vmap[t]
+    mt = mt[(mt >= 0).all(dim=1)]
+    pick = lambda a: None if a is None else torch.as_tensor(a).to(dev).to(torch.float64).reshape(-1, 3)[keep]
+    return v[keep], mt, pick(vertex_colors), pick(vertex_normals)
+
+
 def extract_triangle_mesh(volume, with_colors: Optional[bool] = None) -> TriangleMesh:
     """`volume.extract_triangle_mesh()` for a gs2mesh_b200.tsdf.TSDFVolume."""
     dev = volume.device
     L = _lib.lib()
     with_colors = (volume.color is not None) if with_colors is None else with_colors
     with torch.cuda.device(dev):
-        stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+        stream = _lib.stream(dev)
         nb = volume.num_bricks()  # every brick ever opened = pool slots [0, nb)
         if nb == 0:
             return TriangleMesh(np.zeros((0, 3)), np.zeros((0, 3), np.int64), np.zeros((0, 3)) if with_colors else None,

@@ -23,7 +23,8 @@ import torch
 
 from . import _lib
 from ._lib import ptr
-from .evaluate import PointGrid, _points, _stream, precision_recall_f1
+from .evaluate import PointGrid, _points, precision_recall_f1
+from .mesh import TriangleMesh, remove_vertices_by_mask
 
 ALPHA, BETA, GAMMA = 8.0, 0.5, 1.5  # Yuksel's constants as Open3D sets them
 # csv_headers['MobileBrick'] of gs2mesh_utils/eval_utils.py:14 after 'Scan Name': the order evaluate_single returns
@@ -53,8 +54,7 @@ class Mt19937Stream:
 
 
 def _mesh(vertices, triangles, device=None):
-    v = _points(vertices, device if device is not None else (vertices.device if isinstance(vertices, torch.Tensor) and
-                                                              vertices.is_cuda else torch.device("cuda")))
+    v = _points(vertices, _lib.device(device, vertices))
     t = torch.as_tensor(triangles).to(v.device).to(torch.int64).reshape(-1, 3).contiguous()
     nv = v.shape[0]
     if t.shape[0] and (int(t.min().item()) < 0 or int(t.max().item()) >= nv):
@@ -65,7 +65,7 @@ def _mesh(vertices, triangles, device=None):
 def _areas(v, t):
     a = torch.empty(t.shape[0], dtype=torch.float64, device=v.device)
     with torch.cuda.device(v.device):
-        _lib.check(_lib.lib().gsb_eval_triangle_areas(ptr(v), v.shape[0], ptr(t), t.shape[0], ptr(a), _stream(v.device)))
+        _lib.check(_lib.lib().gsb_eval_triangle_areas(ptr(v), v.shape[0], ptr(t), t.shape[0], ptr(a), _lib.stream(v.device)))
     return a.cpu().numpy()
 
 
@@ -87,7 +87,7 @@ def _uniform(v, t, n_samples, stream):
     b = torch.as_tensor(bounds, device=dev)
     with torch.cuda.device(dev):
         _lib.check(_lib.lib().gsb_eval_sample_uniform(ptr(v), v.shape[0], ptr(t), t.shape[0], ptr(b), ptr(variates),
-                                                      n_samples, ptr(out), _stream(dev)))
+                                                      n_samples, ptr(out), _lib.stream(dev)))
     return out, S
 
 
@@ -119,10 +119,10 @@ def eliminate(points, number_of_points, r_max, r_min, return_info=False):
         kept = torch.arange(M, device=dev)
         return (kept, info) if return_info else kept
     L = _lib.lib()
-    grid = PointGrid(p, min_cell=r_max * 1.001)
+    grid = PointGrid(p, r_max)
     counts = torch.empty(M, dtype=torch.int64, device=dev)
     with torch.cuda.device(dev):
-        s = _stream(dev)
+        s = _lib.stream(dev)
         _lib.check(L.gsb_eval_poisson_neighbours(C.byref(grid.desc), r_max, r_min, ptr(counts), None, None, None, s))
         offsets = torch.zeros(M + 1, dtype=torch.int64, device=dev)
         torch.cumsum(counts, 0, out=offsets[1:])
@@ -170,8 +170,7 @@ def sample_points_poisson_disk(vertices, triangles, number_of_points, init_facto
 def visibility_test(vertices, volume, min_pts, resolution, voxel_size, device=None):
     """evaluate.py:34-41's visibility: device bool [N], True where the nearest voxel of `volume` (reshaped to
     `resolution`, read as D, H, W) is > 0 as a float32, False outside the volume."""
-    v = _points(vertices, device if device is not None else (vertices.device if isinstance(vertices, torch.Tensor) and
-                                                              vertices.is_cuda else torch.device("cuda")))
+    v = _points(vertices, _lib.device(device, vertices))
     dev = v.device
     res = np.asarray(resolution).astype(np.int64).reshape(3)
     vol = np.asarray(volume).reshape(tuple(res)).astype(np.float32) > 0  # torch.from_numpy(volume).float() > 0
@@ -181,30 +180,9 @@ def visibility_test(vertices, volume, min_pts, resolution, voxel_size, device=No
     with torch.cuda.device(dev):
         rc = _lib.lib().gsb_eval_visibility(ptr(v), v.shape[0], (C.c_double * 3)(*mins.tolist()),
                                             float(np.float64(voxel_size)), (C.c_int32 * 3)(*[int(r) for r in res]),
-                                            ptr(vol_d), ptr(keep), _stream(dev))
-    if rc == _lib.GSB_ERR_INVALID:
-        raise ValueError(_lib.lib().gsb_last_error().decode())
-    _lib.check(rc)
+                                            ptr(vol_d), ptr(keep), _lib.stream(dev))
+    _lib.check(rc, invalid_is_value_error=True)
     return keep.bool()
-
-
-def remove_vertices_by_mask(vertices, triangles, vertex_mask, vertex_colors=None, vertex_normals=None):
-    """TriangleMesh.remove_vertices_by_mask(mask): drops the vertices where vertex_mask is True, keeping the rest (and
-    their colours and normals) in order; keeps the triangles whose three vertices survive, in order, re-indexed.
-    Vertices no triangle uses stay.  Returns (vertices, triangles, colours or None, normals or None) as device tensors."""
-    v = torch.as_tensor(vertices)
-    dev = v.device if v.is_cuda else torch.device("cuda")
-    v = v.to(dev).to(torch.float64).reshape(-1, 3)
-    t = torch.as_tensor(triangles).to(dev).to(torch.int64).reshape(-1, 3)
-    keep = ~torch.as_tensor(vertex_mask).to(dev).to(torch.bool).reshape(-1)
-    if keep.shape[0] != v.shape[0]:
-        raise ValueError("remove_vertices_by_mask: the mask must have one entry per vertex")
-    vmap = torch.cumsum(keep.to(torch.int64), 0) - 1
-    vmap = torch.where(keep, vmap, torch.full_like(vmap, -1))
-    mt = vmap[t]
-    mt = mt[(mt >= 0).all(dim=1)]
-    pick = lambda a: None if a is None else torch.as_tensor(a).to(dev).to(torch.float64).reshape(-1, 3)[keep]
-    return v[keep], mt, pick(vertex_colors), pick(vertex_normals)
 
 
 def align_prediction(gt_vertices, pred_vertices):
@@ -225,7 +203,6 @@ def evaluate_single(gt_dir, pred_path, exp_path, scan_name, device="cuda", seed=
     F1@5mm]; writes <exp_path>/<scan_name>_cropped.ply.  One Mt19937Stream(seed) feeds both Poisson-disk samplings, the
     GT's first.  The no-triangle fallback permutes with np.random.RandomState(seed)."""
     from .io import read_triangle_mesh_ply
-    from .mesh import TriangleMesh
 
     dev = torch.device(device)
     if dev.type == "cuda" and dev.index is None:

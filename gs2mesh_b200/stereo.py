@@ -16,7 +16,6 @@ written when the renderer writes images.  There is no CPU fallback.
 """
 from __future__ import annotations
 
-import ctypes as C
 import os
 import sys
 from argparse import Namespace
@@ -49,10 +48,6 @@ def _check_frame(height, width):
         raise ValueError(f"stereo frames must be 1..{MAX_WIDTH} wide and 1..{MAX_HEIGHT} high, not {width}x{height}")
 
 
-def _stream(dev):
-    return C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-
-
 def _cuda(t, dtype, name):
     if not isinstance(t, torch.Tensor):
         t = torch.as_tensor(np.ascontiguousarray(t))
@@ -75,7 +70,7 @@ def pack_inputs(left_u8, right_u8):
     Hp, Wp = padded_shape(H, W)
     out = torch.empty(4, 3, Hp, Wp, dtype=torch.float32, device=left.device)
     with torch.cuda.device(left.device):
-        _lib.check(_lib.lib().gsb_stereo_pack_inputs(ptr(left), ptr(right), W, H, ptr(out), _stream(left.device)))
+        _lib.check(_lib.lib().gsb_stereo_pack_inputs(ptr(left), ptr(right), W, H, ptr(out), _lib.stream(left.device)))
     return out
 
 
@@ -94,7 +89,7 @@ def disparities(flow_lr, flow_rl, height, width, sign):
     d_rl = torch.empty(Hp, Wp, dtype=torch.float32, device=fl.device)
     with torch.cuda.device(fl.device):
         _lib.check(_lib.lib().gsb_stereo_disparities(ptr(fl), ptr(fr), width, height, float(sign), ptr(d_lr), ptr(d_rl),
-                                                     _stream(fl.device)))
+                                                     _lib.stream(fl.device)))
     return d_lr, d_rl
 
 
@@ -132,7 +127,7 @@ def occlusion_depth(disp_lr, disp_rl, threshold, numerator=None, *, want_mask=Tr
     with torch.cuda.device(dl.device):
         _lib.check(_lib.lib().gsb_stereo_occlusion_depth(
             ptr(dl), ptr(dr), W, H, int(dr.shape[1]) if dr is not None else 0, float(threshold),
-            float(numerator) if numerator is not None else 0.0, ptr(visible), ptr(depth), _stream(dl.device)))
+            float(numerator) if numerator is not None else 0.0, ptr(visible), ptr(depth), _lib.stream(dl.device)))
     return visible, depth
 
 

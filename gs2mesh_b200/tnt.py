@@ -28,7 +28,7 @@ import torch
 
 from . import _lib
 from ._lib import ptr
-from .evaluate import PointGrid, _points, _stream
+from .evaluate import PointGrid, _points
 
 # The benchmark's published thresholds (toolbox config.py) for the scenes gs2mesh evaluates.
 SCENES_TAU = {"Barn": 0.01, "Caterpillar": 0.005, "Ignatius": 0.003, "Truck": 0.005}
@@ -107,7 +107,7 @@ def transform_points(points, transformation):
     T = np.ascontiguousarray(np.asarray(transformation, dtype=np.float64).reshape(4, 4))
     with torch.cuda.device(p.device):
         _lib.check(_lib.lib().gsb_eval_transform_points(ptr(p), p.shape[0], T.ctypes.data_as(C.POINTER(C.c_double)),
-                                                        ptr(out), _stream(p.device)))
+                                                        ptr(out), _lib.stream(p.device)))
     return out
 
 
@@ -130,10 +130,8 @@ def crop_point_cloud(points, volume):
     poly_d = torch.as_tensor(poly, device=dev)
     with torch.cuda.device(dev):
         rc = _lib.lib().gsb_eval_crop_polygon(ptr(p), n, ptr(poly_d), len(poly), axis, float(volume.axis_min),
-                                              float(volume.axis_max), ptr(keep), ptr(counter), ptr(host), _stream(dev))
-    if rc == _lib.GSB_ERR_INVALID:
-        raise ValueError(_lib.lib().gsb_last_error().decode())
-    _lib.check(rc)
+                                              float(volume.axis_max), ptr(keep), ptr(counter), ptr(host), _lib.stream(dev))
+    _lib.check(rc, invalid_is_value_error=True)
     return p[keep.bool()]
 
 
@@ -156,10 +154,8 @@ def voxel_down_sample(points, voxel_size):
     dbl3 = C.c_double * 3
     with torch.cuda.device(dev):
         rc = L.gsb_eval_voxel_downsample(ptr(p), n, dbl3(*lo.tolist()), dbl3(*hi.tolist()), float(voxel_size), ptr(ws),
-                                         ws.numel(), ptr(out), ptr(count), _stream(dev))
-    if rc == _lib.GSB_ERR_INVALID:
-        raise ValueError(L.gsb_last_error().decode())
-    _lib.check(rc)
+                                         ws.numel(), ptr(out), ptr(count), _lib.stream(dev))
+    _lib.check(rc, invalid_is_value_error=True)
     return out[:int(count.item())]
 
 
@@ -227,7 +223,7 @@ class _Moments:
         m = None if means is None else (C.c_double * 6)(*[float(x) for x in means])
         with torch.cuda.device(self.dev):
             _lib.check(_lib.lib().gsb_eval_icp_moments(ptr(src), ptr(idx), ptr(d2), src.shape[0], ptr(tgt), pass_, m,
-                                                       ptr(self.ws), ptr(self.out), _stream(self.dev)))
+                                                       ptr(self.ws), ptr(self.out), _lib.stream(self.dev)))
         r = self.out.cpu().numpy()
         return r[:12], int(r[12])
 
@@ -259,7 +255,7 @@ def registration_icp(source, target, threshold, init=None, with_scaling=True, re
         if n:
             with torch.cuda.device(dev):
                 _lib.check(_lib.lib().gsb_eval_icp_correspond(C.byref(grid.desc), ptr(pcd), n, float(threshold), ptr(idx),
-                                                              ptr(d2), _stream(dev)))
+                                                              ptr(d2), _lib.stream(dev)))
         sums, cnt = moments(pcd, idx, d2, tgt, 0)
         if cnt == 0:
             return sums, cnt, 0.0, 0.0
@@ -531,7 +527,7 @@ def run_evaluation(dataset_dir, traj_path, ply_path, out_dir, seed=0, tau=None, 
     print("===========================")
     print("Evaluating %s" % scene)
     print("===========================")
-    dev = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
+    dev = _lib.device(device)
     colmap_ref_logfile = os.path.join(dataset_dir, scene + "_COLMAP_SfM.log")
     alignment = os.path.join(dataset_dir, scene + "_trans.txt")
     gt_filen = os.path.join(dataset_dir, scene + ".ply")

@@ -115,3 +115,7 @@ def test_grid_axis_limit_is_refused(gsb_lib):
         if not ok:
             assert L.gsb_eval_icp_correspond(C.byref(g), fake, 0, 1.0, fake, fake, None) == _lib.GSB_ERR_INVALID
             assert L.gsb_eval_grid_build(C.byref(g), fake, 1 << 30, None) == _lib.GSB_ERR_INVALID
+    # a grid without points: the 27-cell searches would return at once, so only the descriptor check can refuse it
+    g = _lib.GsbPointGrid((C.c_double * 3)(0, 0, 0), 1.0, (C.c_int32 * 3)((1 << 21) + 1, 1, 1), 256, 0, 256, 256)
+    assert L.gsb_eval_radius_downsample(C.byref(g), 0.5, fake, fake, fake, None, None) == _lib.GSB_ERR_INVALID
+    assert L.gsb_eval_poisson_neighbours(C.byref(g), 0.5, 0.0, fake, None, None, None, None) == _lib.GSB_ERR_INVALID
