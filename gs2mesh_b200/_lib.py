@@ -23,6 +23,7 @@ RASTER_PAIR_SHARED_DEPTH = 64
 
 BRICK = 16
 BRICK_VOXELS = 4096
+KNN_MAX_K = 32  # GSB_KNN_MAX_K
 
 _vp = C.c_void_p
 
@@ -101,6 +102,8 @@ SIGNATURES = {
     "gsb_eval_grid_build": (C.c_int, [C.POINTER(GsbPointGrid), _vp, C.c_size_t, _vp]),
     "gsb_eval_nearest": (C.c_int, [C.POINTER(GsbPointGrid), _vp, C.c_int64, C.c_double, _vp, _vp, _vp]),
     "gsb_eval_radius_downsample": (C.c_int, [C.POINTER(GsbPointGrid), C.c_double, _vp, _vp, _vp, C.POINTER(C.c_int32), _vp]),
+    "gsb_eval_knn": (C.c_int, [C.POINTER(GsbPointGrid), _vp, C.c_int64, C.c_int32, _vp, _vp, _vp]),
+    "gsb_eval_estimate_normals": (C.c_int, [C.POINTER(GsbPointGrid), _vp, C.c_int64, C.c_int32, _vp, _vp]),
     "gsb_eval_transform_points": (C.c_int, [_vp, C.c_int64, C.POINTER(C.c_double), _vp, _vp]),
     "gsb_eval_crop_polygon": (C.c_int, [_vp, C.c_int64, _vp, C.c_int32, C.c_int32, C.c_double, C.c_double, _vp, _vp, _vp, _vp]),
     "gsb_eval_voxel_workspace_bytes": (C.c_size_t, [C.c_int64]),

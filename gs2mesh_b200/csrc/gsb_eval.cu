@@ -135,76 +135,28 @@ __global__ void __launch_bounds__(256) grid_scatter_kernel(const GsbPointGrid g,
   g.ids[g.cell_start[c] + atomicAdd(&fill[c], 1u)] = i;
 }
 
-// Rings of cells at Chebyshev distance k around the query's cell.  Every point in a ring > k lies at least k*h away, so
-// the search stops once the best distance is below that bound, or once k*h reaches max_dist.  Returns the nearest point
-// (lowest index among equal squared distances; -1 if none) and its ((dx*dx)+dy*dy)+dz*dz; a point at max_dist or beyond
-// may be missed.  A query with a coordinate that is not finite returns (+inf, -1) without searching.
-//
-// The query's cell is clamped, in double, to [-kFarCells, dims-1 + kFarCells] per axis: a query farther out gets a cell
-// nearer the grid, which only shrinks the ring bounds (k-1)*h, so they stay lower bounds; k and qc +- k stay far from
-// int64 overflow, and the rings walked stay within kFarCells + dims.
-//
-// The ring bound's relative margin kRingMargin must exceed the rounding error of the cell indices.  A query's or a
-// point's index (p - o) / h rounds twice, so it is off by at most 2^-52 * |index| cells.  A point in ring k of a query
-// has |index| < dims and the query |index| <= k + dims, so the two are off by at most 2^-52 * (k + 2*dims) cells, which
-// stays below kRingMargin * (k - 1) for every k >= 2 while dims <= kMaxAxisCells (9.3e-10 at k = 2; gsb_grid.cuh's
-// grid_ok refuses larger axes).  The distance expression's own rounding (a few ulp) is far below the margin.  PointGrid's
-// cell floor of (hi - lo) / 1e6 keeps every axis at about 1e6 cells: a change to that floor must keep it within the limit.
-constexpr double kFarCells = 1099511627776.0;  // 2^40
-constexpr double kRingMargin = 1e-9;
-
+// The rings of gsb_grid.cuh's walk_rings: the search stops once the best squared distance is below the next ring's bound,
+// or once that bound reaches max_dist.  Returns the nearest point (lowest index among equal squared distances; -1 if none)
+// and its ((dx*dx)+dy*dy)+dz*dz; a point at max_dist or beyond may be missed.  A query with a coordinate that is not
+// finite returns (+inf, -1) without searching.
 struct Nearest {
   double d2;
   long long id;
 };
 
-__device__ __forceinline__ long long query_cell(double p, double o, double h, int dim) {
-  return (long long)fmin(fmax(floor((p - o) / h), -kFarCells), (double)(dim - 1) + kFarCells);
-}
-
 __device__ __forceinline__ Nearest ring_nearest(const GsbPointGrid& g, double qx, double qy, double qz, double max_dist) {
   if (!(isfinite(qx) && isfinite(qy) && isfinite(qz))) return {INFINITY, -1};
-  const long long qc[3] = {query_cell(qx, g.origin[0], g.cell, g.dims[0]), query_cell(qy, g.origin[1], g.cell, g.dims[1]),
-                           query_cell(qz, g.origin[2], g.cell, g.dims[2])};
-  // first ring that can reach the grid, last ring that still meets it
-  long long k0 = 0, k1 = 0;
-#pragma unroll
-  for (int a = 0; a < 3; ++a) {
-    const long long below = -qc[a], above = qc[a] - (g.dims[a] - 1);
-    k0 = max(k0, max(below, above));
-    k1 = max(k1, max(qc[a], (long long)(g.dims[a] - 1) - qc[a]));
-  }
   double best2 = INFINITY;
   long long best = -1;
-  const double margin = 1.0 - kRingMargin;
-  for (long long k = k0; k <= k1; ++k) {
-    const double lb = (double)(k > 0 ? k - 1 : 0) * g.cell * margin;  // every point of ring k is at least this far away
-    if (lb >= max_dist) break;
-    if (best >= 0 && best2 < lb * lb) break;
-    const long long xl = max(qc[0] - k, 0ll), xh = min(qc[0] + k, (long long)g.dims[0] - 1);
-    const long long yl = max(qc[1] - k, 0ll), yh = min(qc[1] + k, (long long)g.dims[1] - 1);
-    for (long long x = xl; x <= xh; ++x) {
-      const bool xedge = (x == qc[0] - k) || (x == qc[0] + k);
-      for (long long y = yl; y <= yh; ++y) {
-        const bool yedge = xedge || (y == qc[1] - k) || (y == qc[1] + k);
-        // edge rows of the ring are whole z runs (clamped to the grid); inner rows only touch its two z faces
-        const long long zl = yedge ? max(qc[2] - k, 0ll) : qc[2] - k;
-        const long long zh = yedge ? min(qc[2] + k, (long long)g.dims[2] - 1) : qc[2] + k;
-        for (long long zz = zl; zz <= zh; zz += (yedge ? 1 : 2 * k)) {
-          if (zz < 0 || zz >= g.dims[2]) continue;
-          const long long c = (x * g.dims[1] + y) * g.dims[2] + zz;
-          for (long long s = g.cell_start[c], e = g.cell_start[c + 1]; s < e; ++s) {
-            const long long id = g.ids[s];
-            const double d2 = sq_dist(qx, qy, qz, g.points + 3 * id);
-            if (d2 < best2 || (d2 == best2 && id < best)) {
-              best2 = d2;
-              best = id;
-            }
-          }
+  walk_rings(
+      g, qx, qy, qz, max_dist, [&](double lb) { return best >= 0 && best2 < lb * lb; },
+      [&](long long id) {
+        const double d2 = sq_dist(qx, qy, qz, g.points + 3 * id);
+        if (d2 < best2 || (d2 == best2 && id < best)) {
+          best2 = d2;
+          best = id;
         }
-      }
-    }
-  }
+      });
   return {best2, best};
 }
 

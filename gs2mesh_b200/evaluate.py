@@ -63,7 +63,7 @@ def grid_layout(lo, hi, core, n, cells_per_point=4.0, min_cell=0.0, max_cells=1 
     """(cell, dims) of PointGrid for n points with bounds lo / hi and 1%..99% quantile extent `core` per axis.
 
     The cell never falls below (hi - lo).max() * 1e-6, so no axis has more than about 1e6 cells: the ring search's
-    rounding margin (gsb_eval.cu, kRingMargin) covers up to 2^21 (gsb_grid.cuh, kMaxAxisCells).  When the points coincide
+    rounding margin (gsb_grid.cuh, kRingMargin) covers up to 2^21 (gsb_grid.cuh, kMaxAxisCells).  When the points coincide
     (an extent of 1e-294 or less) the cell is tied to the coordinates' magnitude instead, max(|lo|, |hi|, 1) * 2^-30: one
     cell holds them all, and the cell stays a normal number, so the search's distance bounds keep their precision."""
     lo, hi, core = (np.asarray(x, dtype=np.float64) for x in (lo, hi, core))
@@ -126,6 +126,27 @@ class PointGrid:
             _lib.check(_lib.lib().gsb_eval_nearest(C.byref(self.desc), ptr(q), n, float(max_dist), ptr(dist), ptr(idx),
                                                    _stream(dev)))
         return dist, idx
+
+    def knn(self, queries, k):
+        """The k nearest grid points of every query -> (d2 fp64 [N,k], idx int64 [N,k]) on the device (gsb_eval_knn):
+        d2 = ((dx*dx)+dy*dy)+dz*dz in ascending (d2, index) order, rows padded with (+inf, -1) past the grid's size, and
+        only padding for a query with a NaN or infinite coordinate.  k is 1..32."""
+        k = int(k)
+        if not 1 <= k <= _lib.KNN_MAX_K:
+            raise ValueError(f"knn: k must be in 1..{_lib.KNN_MAX_K}, not {k}")
+        q = _points(queries, self.points.device)
+        dev = q.device
+        n = q.shape[0]
+        d2 = torch.empty(n, k, dtype=torch.float64, device=dev)
+        idx = torch.empty(n, k, dtype=torch.int64, device=dev)
+        with torch.cuda.device(dev):
+            _lib.check(_lib.lib().gsb_eval_knn(C.byref(self.desc), ptr(q), n, k, ptr(d2), ptr(idx), _stream(dev)))
+        return d2, idx
+
+
+def knn(queries, reference, k):
+    """Exact k nearest neighbours of every query among `reference`: PointGrid(reference).knn(queries, k)."""
+    return PointGrid(reference).knn(queries, k)
 
 
 def nearest(queries, reference, max_dist=math.inf):

@@ -233,18 +233,23 @@ def read_triangle_mesh_ply(path, with_colors=False):
     return xyz, tris, colors
 
 
-def write_point_cloud_ply(path, points, colors=None):
+def write_point_cloud_ply(path, points, colors=None, normals=None):
     """o3d.io.write_point_cloud for eval.py's visualisation clouds (eval.py:21-25): binary little-endian, double xyz,
-    uchar rgb = round(255 * colour)."""
+    double normals nx ny nz when given, uchar rgb = round(255 * colour), in Open3D's property order."""
     points = np.asarray(points, dtype=np.float64).reshape(-1, 3)
     props = [("x", "<f8"), ("y", "<f8"), ("z", "<f8")]
     header = ["ply", "format binary_little_endian 1.0", f"element vertex {len(points)}", "property double x",
               "property double y", "property double z"]
+    if normals is not None:
+        props += [("nx", "<f8"), ("ny", "<f8"), ("nz", "<f8")]
+        header += ["property double nx", "property double ny", "property double nz"]
     if colors is not None:
         props += [("red", "u1"), ("green", "u1"), ("blue", "u1")]
         header += ["property uchar red", "property uchar green", "property uchar blue"]
     tab = np.zeros(len(points), dtype=props)
     tab["x"], tab["y"], tab["z"] = points.T
+    if normals is not None:
+        tab["nx"], tab["ny"], tab["nz"] = np.asarray(normals, dtype=np.float64).reshape(-1, 3).T
     if colors is not None:
         rgb = np.clip(np.rint(np.asarray(colors, dtype=np.float64).reshape(-1, 3) * 255.0), 0, 255).astype(np.uint8)
         tab["red"], tab["green"], tab["blue"] = rgb.T

@@ -9,8 +9,8 @@ Restated (file:line under evaluation/TNT/eval_code/python_toolbox/evaluation):
   plot.py:40-109           plot_graph (only when matplotlib is installed)
 
 The Open3D 0.17 operations underneath (PointCloud.Transform, CropInPolygon, VoxelDownSample, RegistrationICP with
-TransformationEstimationPointToPoint) are gsb_eval_* kernels of include/gs2mesh_b200.h (gs2mesh_b200/csrc/gsb_tnt.cu,
-gsb_eval.cu); DESIGN.md section 7d gives their operation orders.  Host work per ICP iteration is the 3x3 SVD and two
+TransformationEstimationPointToPoint, EstimateNormals) are gsb_eval_* kernels of include/gs2mesh_b200.h
+(gs2mesh_b200/csrc/gsb_tnt.cu, gsb_eval.cu, gsb_normals.cu); DESIGN.md section 7d gives their operation orders.  Host work per ICP iteration is the 3x3 SVD and two
 reads of 13 moments.  There is no CPU fallback.  The rough RANSAC alignment runs on the host over the camera centres
 with a seeded generator: it is the one step that cannot equal Open3D's bits (its random sequence is not reproducible).
 """
@@ -164,6 +164,25 @@ def uniform_down_sample(points, every_k_points):
     if int(every_k_points) <= 0:
         raise ValueError("uniform_down_sample: every_k_points must be positive")
     return _points(points)[::int(every_k_points)].contiguous()
+
+
+def estimate_normals(points, knn=20):
+    """PointCloud.estimate_normals(KDTreeSearchParamKNN(knn)) for a cloud without normals (Open3D 0.17, with
+    fast_normal_computation): per point, the covariance of its knn nearest points (itself included; the identity for
+    fewer than 3), FastEigen3x3's eigenvector of the smallest eigenvalue, (0, 0, 1) where that is zero.  Not oriented.
+    fp64 [N,3] on the points' device (gsb_eval_estimate_normals); knn is 1..32."""
+    p = _points(points)
+    knn = int(knn)
+    if not 1 <= knn <= _lib.KNN_MAX_K:
+        raise ValueError(f"estimate_normals: knn must be in 1..{_lib.KNN_MAX_K}, not {knn}")
+    out = torch.empty_like(p)
+    if p.shape[0] == 0:
+        return out
+    grid = PointGrid(p)
+    with torch.cuda.device(p.device):
+        _lib.check(_lib.lib().gsb_eval_estimate_normals(C.byref(grid.desc), ptr(p), p.shape[0], knn, ptr(out),
+                                                        _lib.stream(p.device)))
+    return out
 
 
 def compute_point_cloud_distance(source, target):
@@ -448,9 +467,9 @@ def _matplotlib():
         return None
 
 
-def write_color_distances(path, points, distances, max_distance):
-    """evaluation.py:48-55 without normals: hot_r(min(d, max) / max), written with Open3D's ColorToUint8 rounding.
-    Needs matplotlib (returns None without it)."""
+def write_color_distances(path, points, distances, max_distance, normals=None):
+    """evaluation.py:48-55: hot_r(min(d, max) / max), written with Open3D's ColorToUint8 rounding, and the normals (x y z
+    nx ny nz red green blue) when given.  Needs matplotlib (returns None without it)."""
     plt = _matplotlib()
     if plt is None:
         return None
@@ -459,7 +478,7 @@ def write_color_distances(path, points, distances, max_distance):
 
     colors = plt.get_cmap("hot_r")(np.minimum(np.asarray(distances), max_distance) / max_distance)[:, :3]
     # write_point_cloud_ply rounds colour*255 with np.rint; pass colours already on Open3D's uint8 grid
-    return write_point_cloud_ply(path, points, color_to_uint8(colors) / 255.0)
+    return write_point_cloud_ply(path, points, color_to_uint8(colors) / 255.0, normals)
 
 
 def plot_graph(scene, fscore, dist_threshold, edges_source, cum_source, edges_target, cum_target, plot_stretch,
@@ -491,13 +510,18 @@ def plot_graph(scene, fscore, dist_threshold, edges_source, cum_source, edges_ta
 def evaluate_histo(source, target, trans, crop_volume, voxel_size, threshold, filename_mvs, plot_stretch, scene_name,
                    verbose=True):
     """evaluation.py:60-160 (EvaluateHisto).  Writes <scene>.recall.txt, .precision.txt and .prf_tau_plotstr.txt, and the
-    coloured <scene>.precision.ply / .recall.ply when matplotlib is installed (without the toolbox's normals)."""
+    coloured <scene>.precision.ply / .recall.ply with the toolbox's normals (estimate_normals, knn = 20) when matplotlib
+    is installed."""
     s = voxel_down_sample(crop_point_cloud(transform_points(source, trans), crop_volume), voxel_size)
     t = voxel_down_sample(crop_point_cloud(_points(target, s.device), crop_volume), voxel_size)
+    s_normals = estimate_normals(s, 20).cpu().numpy()
+    t_normals = estimate_normals(t, 20).cpu().numpy()
     distance1 = compute_point_cloud_distance(s, t).cpu().numpy()
     distance2 = compute_point_cloud_distance(t, s).cpu().numpy()
-    write_color_distances(filename_mvs + "/" + scene_name + ".precision.ply", s.cpu().numpy(), distance1, 3 * threshold)
-    write_color_distances(filename_mvs + "/" + scene_name + ".recall.ply", t.cpu().numpy(), distance2, 3 * threshold)
+    write_color_distances(filename_mvs + "/" + scene_name + ".precision.ply", s.cpu().numpy(), distance1, 3 * threshold,
+                          s_normals)
+    write_color_distances(filename_mvs + "/" + scene_name + ".recall.ply", t.cpu().numpy(), distance2, 3 * threshold,
+                          t_normals)
     r = get_f1_score_histo2(threshold, filename_mvs, plot_stretch, distance1, distance2)
     precision, recall, fscore, _, cum_source, _, cum_target = r
     np.savetxt(filename_mvs + "/" + scene_name + ".recall.txt", cum_target)

@@ -393,6 +393,26 @@ int gsb_eval_nearest(const GsbPointGrid* grid, const double* queries, int64_t n_
 int gsb_eval_radius_downsample(const GsbPointGrid* grid, double radius, uint8_t* keep, uint32_t* counters,
                                uint32_t* host_undecided, int32_t* rounds, void* stream);
 
+/* k nearest neighbours and normal estimation on the grid (gsb_normals.cu).  k is at most GSB_KNN_MAX_K: each thread
+ * keeps its k best candidates in local memory.  Calls with k outside 1..GSB_KNN_MAX_K, a negative count or a missing
+ * pointer are refused (GSB_ERR_INVALID) before anything is enqueued.
+ *   gsb_eval_knn               the k nearest grid points of each query, exact: row i of dist2 / index (device double /
+ *                              int64 [n_queries, k]) holds ((dx*dx)+dy*dy)+dz*dz and the point's index in ascending
+ *                              (dist2, index) order, so among equal squared distances the lower index comes first, at
+ *                              the k-th place too.  Rows of grids with fewer than k points end in (+inf, -1); a query
+ *                              with a NaN or infinite coordinate gets only (+inf, -1).
+ *   gsb_eval_estimate_normals  Open3D 0.17 PointCloud::EstimateNormals(KDTreeSearchParamKNN(k)) with
+ *                              fast_normal_computation, for a cloud without normals: per point (device double [n,3]),
+ *                              the covariance of its gsb_eval_knn neighbours (the point itself included when it is a
+ *                              grid point; the identity for fewer than 3), the eigenvector of its smallest eigenvalue by
+ *                              FastEigen3x3, and (0, 0, 1) where that is zero.  No orientation.  normals: device double
+ *                              [n,3].  DESIGN.md section 7d gives the operation order. */
+#define GSB_KNN_MAX_K 32
+int gsb_eval_knn(const GsbPointGrid* grid, const double* queries, int64_t n_queries, int32_t k, double* dist2,
+                 int64_t* index, void* stream);
+int gsb_eval_estimate_normals(const GsbPointGrid* grid, const double* points, int64_t n_points, int32_t k, double* normals,
+                              void* stream);
+
 /* Tanks and Temples evaluation (evaluation/TNT/eval_code/python_toolbox/evaluation), restating Open3D 0.17's
  * PointCloud::Transform, SelectionPolygonVolume::CropInPolygon, VoxelDownSample and RegistrationICP with
  * TransformationEstimationPointToPoint (Eigen::umeyama); DESIGN.md section 7d gives each operation order.

@@ -78,6 +78,7 @@ def main():
         gt_pcd = torch.as_tensor(gt, device=dev)
         # warm-up of every kernel and allocation shape at a small size
         tnt.registration_vol_ds(pcd[:100000], gt_pcd[:400000], gt_trans, vol, tau, 80 * tau, 20, verbose=False)
+        tnt.estimate_normals(pcd[:100000], 20)
         stages = {}
         T0, stages["alignment_ms"] = timed(lambda: tnt.trajectory_alignment(None, traj, traj, gt_trans, seed=args.seed))
         r2, stages["vol_ds_1_ms"] = timed(lambda: tnt.registration_vol_ds(pcd, gt_pcd, T0, vol, tau, tau * 80, 20,
@@ -88,6 +89,9 @@ def main():
                                                                    verbose=False))
         res, stages["histo_ms"] = timed(lambda: tnt.evaluate_histo(pcd, gt_pcd, r.transformation, vol, tau / 2, tau, tmp, 5,
                                                                    "Synth"))
+        # the normals evaluate_histo estimates, alone: the downsampled GT (the larger of its two clouds), grid included
+        t_ds = tnt.voxel_down_sample(tnt.crop_point_cloud(gt_pcd, vol), tau / 2)
+        _, stages["normals_gt_ms"] = timed(lambda: tnt.estimate_normals(t_ds, 20))
         # the whole run_evaluation from files, PLY reads included
         d = os.path.join(tmp, "Synth")
         os.makedirs(d)
@@ -107,6 +111,7 @@ def main():
     name, power = _card()
     print(json.dumps({"card": name, "power_limit": power, "recon_points": args.recon, "gt_points": args.gt, "tau": tau,
                       "icp_iterations": [r2.iterations, r3.iterations, r.iterations], "precision_recall_fscore": eva,
+                      "normals_gt_points": int(t_ds.shape[0]),
                       **{k: round(v, 2) for k, v in stages.items()}}))
 
 
