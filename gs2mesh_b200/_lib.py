@@ -66,7 +66,6 @@ SIGNATURES = {
     "gsb_raster_workspace_bytes": (C.c_size_t, [C.c_int32, C.c_int32, C.c_int32, C.c_int64]),
     "gsb_raster_forward": (C.c_int, [C.POINTER(GsbRasterArgs), _vp]),
     "gsb_raster_forward_pair": (C.c_int, [C.POINTER(GsbRasterArgs), C.POINTER(GsbRasterArgs), _vp, _vp]),
-    "gsb_raster_required_instances": (C.c_int64, []),
     "gsb_raster_mark_visible": (C.c_int, [C.c_int32, _vp, _vp, _vp, _vp, _vp]),
     "gsb_image_to_u8": (C.c_int, [_vp, C.c_int32, C.c_int32, _vp, _vp]),
     "gsb_tsdf_create": (_vp, [C.POINTER(GsbVolumeDesc)]),

@@ -39,12 +39,10 @@ namespace gsb {
 
 thread_local char g_error[512] = {0};
 std::atomic<uint64_t> g_launches{0};
-std::atomic<bool> g_blend_trace_on{false};
 Profiler g_prof;
 static const char* kStageNames[kStCount] = {"preprocess", "depth_sort", "emit", "tile_sort", "tile_ranges",
                                             "render",     "to_u8", "prepare_depth", "mark_bricks", "integrate",
                                             "merge_index", "merge_pack", "merge_reduce", "merge_unpack"};
-static thread_local int64_t g_required_instances = 0;
 
 namespace {
 
@@ -1291,17 +1289,6 @@ __device__ __forceinline__ unsigned long long pack_f32x2(float lo, float hi) {
 // One CTA per tile in the hardware's block order: it mixes long and short lists on every SM, so the gather latency of the
 // short ones hides behind the arithmetic of the long ones; a queue sorted by list length would end the kernel in a long
 // phase of latency-bound tiles, and a persistent grid would keep the kernels of the other in-flight views off the SMs.
-// profiling aid (scripts/blend_trace.py): the <true> instantiation writes, per warp, start / end %globaltimer, list length /
-// records walked, clock cycles spent in (test + slot build, blend loop, waiting for the next chunk's gather) and the
-// number of records blended to trace[(tile * 4 + block) * 8 + 0..6].  The product launch is <false>: no trace code in it.
-__device__ unsigned long long* g_blend_trace = nullptr;
-__device__ __forceinline__ unsigned long long global_timer_ns() {
-  unsigned long long t;
-  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-  return t;
-}
-
-template <bool kTrace>
 __global__ void __launch_bounds__(kTilePixels / 2, 7)
     render_table_kernel(const uint2* __restrict__ ranges, const uint32_t* __restrict__ point_list, int W, int H,
                         const float4* __restrict__ recA, const float4* __restrict__ recB, const float2* __restrict__ recC,
@@ -1325,12 +1312,6 @@ __global__ void __launch_bounds__(kTilePixels / 2, 7)
     uint2 range = ranges[tile];
     if (range.y <= range.x || (int64_t)range.y > capacity) range = make_uint2(0u, 0u);
     const int total = range.y - range.x;
-    unsigned long long* trace = nullptr;
-    uint32_t cyc_build = 0, cyc_blend = 0, cyc_wait = 0, hits = 0;
-    if (kTrace) {
-      trace = g_blend_trace + ((size_t)tile * 4 + warp) * 8;
-      if (lane == 0) trace[0] = global_timer_ns();
-    }
     const bool inside0 = pix_x < (uint32_t)W && pix_y < (uint32_t)H, inside1 = pix_x < (uint32_t)W && pix_y + 4 < (uint32_t)H;
     // the sign of T is the pixel's "done" flag
     unsigned long long TT = pack_f32x2(inside0 ? 1.0f : -1.0f, inside1 ? 1.0f : -1.0f);
@@ -1358,11 +1339,8 @@ __global__ void __launch_bounds__(kTilePixels / 2, 7)
       const float4 Q = lds128(a0 + kTabC + off);  // r, g, b, z
       blend_stage_apply(al, Q.x, Q.y, Q.z, Q.w, TT, C00, C10, C20, Dz0, C01, C11, C21, Dz1);
     };
-    int c0 = 0;
-    for (; c0 < total; c0 += 32) {
+    for (int c0 = 0; c0 < total; c0 += 32) {
       if (__all_sync(0xffffffffu, (TT & 0x8000000080000000ull) == 0x8000000080000000ull)) break;  // both pixels done
-      uint32_t tk0 = 0, tk1 = 0, tk2 = 0;
-      if (kTrace) tk0 = (uint32_t)clock64();
       const int nxt = c0 + 32 + lane;
       if (nxt < total) {  // next chunk's gathers fly while this one is tested and blended
         nA = recA[g_next];
@@ -1394,11 +1372,6 @@ __global__ void __launch_bounds__(kTilePixels / 2, 7)
         sts128(dst + kTabC, make_float4(cB.w, cC.x, cC.y, cA.z));
         sts128(dst + kTabThr, make_float4(l2o, 0.f, 0.f, 0.f));
       }
-      if (kTrace) {
-        __syncwarp();
-        tk1 = (uint32_t)clock64();
-        hits += n;
-      }
       if (n != 0) {  // (a chunk none of whose records reaches the block costs no more than the test)
         if ((n & 1) && lane < kTabSlotBytes / 16) {  // odd count: sentinel after the last hit, u' = -1e30 -> alpha 0 -> skipped
           const float big = lane < 4 ? -1.0e30f : 0.f;  // quads 0..3 = the X table: (u', v, u', v)
@@ -1418,25 +1391,9 @@ __global__ void __launch_bounds__(kTilePixels / 2, 7)
         }
         __syncwarp();  // every lane is done reading before the next chunk overwrites the slots
       }
-      if (kTrace) tk2 = (uint32_t)clock64();
       cA = nA;
       cB = nB;
       cC = nC;
-      if (kTrace) {  // the moves above wait for the gather: touch the values so the wait is inside the bracket
-        const float touch = cA.x + cB.x + cC.x;
-        const uint32_t tk3 = (uint32_t)clock64() + (touch == 1.2345e-30f ? 1u : 0u);
-        cyc_build += tk1 - tk0;
-        cyc_blend += tk2 - tk1;
-        cyc_wait += tk3 - tk2;
-      }
-    }
-    if (kTrace && lane == 0) {
-      trace[1] = global_timer_ns();
-      trace[2] = ((unsigned long long)(uint32_t)total << 32) | (uint32_t)min(c0, total);
-      trace[3] = cyc_build;
-      trace[4] = cyc_blend;
-      trace[5] = cyc_wait;
-      trace[6] = hits;
     }
     const size_t plane = (size_t)H * W;
     const float Tf0 = fabsf(__uint_as_float((uint32_t)TT)), Tf1 = fabsf(__uint_as_float((uint32_t)(TT >> 32)));
@@ -1594,16 +1551,6 @@ extern "C" {
 const char* gsb_last_error(void) { return g_error; }
 int gsb_version(void) { return GSB_VERSION; }
 uint64_t gsb_kernel_launch_count(void) { return g_launches.load(); }
-
-// profiling aid, not part of the reference-facing surface: per-warp timeline of the table blend
-// (device buffer of tiles * 4 * 8 uint64; NULL = off)
-int gsb_debug_blend_trace(void* device_buffer) {
-  unsigned long long* p = static_cast<unsigned long long*>(device_buffer);
-  GSB_CUDA_OK(cudaMemcpyToSymbol(g_blend_trace, &p, sizeof(p)));
-  g_blend_trace_on.store(p != nullptr);
-  return GSB_OK;
-}
-int64_t gsb_raster_required_instances(void) { return g_required_instances; }
 
 int gsb_profile_num_stages(void) { return kStCount; }
 const char* gsb_profile_stage_name(int stage) { return stage >= 0 && stage < kStCount ? kStageNames[stage] : ""; }
@@ -1830,10 +1777,8 @@ static int render_frame_impl(const Frame& f, const uint32_t* point_list, cudaStr
                                                        a->out_color, a->out_depth, a->out_final_T, cap)
     if (!(a->flags & GSB_RASTER_FAST_EXP)) {
       GSB_LAUNCH_RENDER(render_compact_kernel);
-    } else if (g_blend_trace_on.load()) {
-      GSB_LAUNCH_RENDER(render_table_kernel<true>);
     } else {
-      GSB_LAUNCH_RENDER(render_table_kernel<false>);
+      GSB_LAUNCH_RENDER(render_table_kernel);
     }
 #undef GSB_LAUNCH_RENDER
   }
@@ -1848,7 +1793,6 @@ static int finish_sync(const Frame& f, cudaStream_t stream) {
   unsigned long long host_counters[4] = {0, 0, 0, 0};
   GSB_CUDA_OK(cudaMemcpyAsync(host_counters, f.ws.counters, sizeof(host_counters), cudaMemcpyDeviceToHost, stream));
   GSB_CUDA_OK(cudaStreamSynchronize(stream));
-  g_required_instances = (int64_t)host_counters[1];
   if (host_counters[2])
     return fail(GSB_ERR_WORKSPACE, "frame needs %lld instances, workspace sized for %lld", (long long)host_counters[1],
                 (long long)f.cap);
@@ -1876,7 +1820,6 @@ static int cub_path(const Frame& f, cudaStream_t stream) {
   GSB_CUDA_OK(cudaMemcpyAsync(&R32, ws.offsets + (P - 1), sizeof(uint32_t), cudaMemcpyDeviceToHost, stream));
   GSB_CUDA_OK(cudaStreamSynchronize(stream));
   const int64_t R = (int64_t)R32;
-  g_required_instances = R;
   if (R > cap)
     return fail(GSB_ERR_WORKSPACE, "frame needs %lld instances, workspace sized for %lld", (long long)R, (long long)cap);
   if (R > 0) {

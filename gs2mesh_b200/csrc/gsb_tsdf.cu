@@ -588,14 +588,11 @@ bool invert4(const double* m, double* out) {
   return true;
 }
 
-int g_num_sms = 0;
+// SM count of the current device, which sizes the persistent grids launched on it
 int num_sms() {
-  if (g_num_sms == 0) {
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
-      g_num_sms = 132;
-  }
-  return g_num_sms;
+  int dev = 0, n = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) return 132;
+  return n;
 }
 
 }  // namespace
@@ -756,7 +753,8 @@ int gsb_tsdf_integrate(GsbVolume* vol, const float* depth, const uint8_t* rgb, i
   f.W = width;
   f.H = height;
   f.unit_length = unit_length;
-  const int grid = (int)((size_t)num_sms() * 8 < (size_t)d.pool_bricks ? (size_t)num_sms() * 8 : (size_t)d.pool_bricks);
+  const size_t resident = (size_t)num_sms() * 8;
+  const int grid = (int)(resident < (size_t)d.pool_bricks ? resident : (size_t)d.pool_bricks);
   const unsigned long long* hkeys = reinterpret_cast<const unsigned long long*>(d.hash_keys);
   {
     StageTimer tm(kStIntegrate, stream);

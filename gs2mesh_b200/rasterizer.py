@@ -27,18 +27,21 @@ MIN_GUESS = 1 << 20
 
 
 class _Scratch:
-    """Grow-only workspace + binning capacity."""
+    """Grow-only workspace + binning capacity, and the instance counts of calls that do not ask for them."""
 
     def __init__(self, device):
         self.device = device
         self.buf: Optional[torch.Tensor] = None
         self.max_instances = 0
         self.key = None
+        self.counts = torch.zeros(4, dtype=torch.int64, device=device)
 
-    def ensure(self, P, W, H, max_instances):
+    def ensure(self, P, W, H, min_instances):
+        """Workspace for a P-Gaussian W x H frame with room for at least `min_instances` instances; the capacity of a
+        frame shape never shrinks."""
         key = (P, W, H)
+        max_instances = max(self.max_instances if key == self.key else 0, GUESS_PER_GAUSSIAN * P, MIN_GUESS, int(min_instances))
         if self.buf is None or key != self.key or max_instances > self.max_instances:
-            max_instances = max(max_instances, self.max_instances if key == self.key else 0)
             need = _lib.lib().gsb_raster_workspace_bytes(P, W, H, max_instances)
             if self.buf is None or self.buf.numel() < need:
                 self.buf = None  # release before re-allocating
@@ -127,25 +130,24 @@ def rasterize_forward(*, means3D, opacities, viewmatrix, projmatrix, campos, bg,
         radii = torch.empty(P, dtype=torch.int32, device=device) if want_radii else None
         counts = counts_out if counts_out is not None else (torch.zeros(4, dtype=torch.int64, device=device) if want_counts else None)
         scratch = _scratch_for(device)
-        guess = max(scratch.max_instances if scratch.key == (P, W, H) else 0, GUESS_PER_GAUSSIAN * P, MIN_GUESS, int(min_instances))
+        status = counts if counts is not None else scratch.counts  # [0] is the frame's instance need, also on overflow
         stream = C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
         L = _lib.lib()
         if async_mode:
             flags = int(flags) | _lib.RASTER_ASYNC
         for attempt in range(1 if async_mode else 3):
-            ws = scratch.ensure(P, W, H, guess)
+            ws = scratch.ensure(P, W, H, min_instances)
             args = GsbRasterArgs(
                 P=P, sh_degree=int(sh_degree), sh_coeffs=M, width=W, height=H, background=ptr(bg), means3D=ptr(means3D),
                 shs=ptr(shs), colors_precomp=ptr(colors_precomp), opacities=ptr(opacities), scales=ptr(scales),
                 rotations=ptr(rotations), cov3D_precomp=ptr(cov3D_precomp), scale_modifier=float(scale_modifier),
                 viewmatrix=ptr(viewmatrix), projmatrix=ptr(projmatrix), cam_pos=ptr(campos), tan_fovx=float(tan_fovx),
                 tan_fovy=float(tan_fovy), prefiltered=int(bool(prefiltered)), flags=int(flags), out_color=ptr(color),
-                out_depth=ptr(depth), out_final_T=ptr(final_T), radii=ptr(radii), num_rendered=ptr(counts),
+                out_depth=ptr(depth), out_final_T=ptr(final_T), radii=ptr(radii), num_rendered=ptr(status),
                 workspace=ptr(ws), workspace_bytes=ws.numel(), max_instances=scratch.max_instances)
             rc = L.gsb_raster_forward(C.byref(args), stream)
             if rc == _lib.GSB_ERR_WORKSPACE and attempt < 2 and not async_mode:
-                need = int(L.gsb_raster_required_instances())
-                guess = max(int(need * 1.25) + 1024, guess)
+                min_instances = int(int(status[0]) * 1.25) + 1024
                 continue
             _lib.check(rc)
             break
@@ -178,8 +180,7 @@ def rasterize_forward_pair(*, means3D, opacities, shs, scales, rotations, sh_deg
         blocks = []
         for s_, (eye, st) in enumerate(zip(eyes, streams)):
             scratch = _scratch_for(device, st, s_)
-            guess = max(scratch.max_instances if scratch.key == (P, W, H) else 0, GUESS_PER_GAUSSIAN * P, MIN_GUESS, int(min_instances))
-            ws = scratch.ensure(P, W, H, guess)
+            ws = scratch.ensure(P, W, H, min_instances)
             fl = int(flags) | _lib.RASTER_ASYNC | (_lib.RASTER_PAIR_SHARED_DEPTH if shared_depth else 0)
             blocks.append(GsbRasterArgs(
                 P=P, sh_degree=int(sh_degree), sh_coeffs=M, width=W, height=H, background=ptr(bg), means3D=ptr(means3D),

@@ -42,7 +42,7 @@ enum {
   GSB_ERR_INVALID = 1,    /* bad argument combination (mirrors the Python Exceptions in
                              DGR/diff_gaussian_rasterization/__init__.py:191-195 and
                              AT_ERROR in rasterize_points.cu:57-59)                        */
-  GSB_ERR_WORKSPACE = 2,  /* caller workspace too small; see gsb_raster_required_instances */
+  GSB_ERR_WORKSPACE = 2,  /* caller workspace too small; num_rendered[0] tells the need   */
   GSB_ERR_CUDA = 3,       /* CUDA runtime / launch error                                  */
   GSB_ERR_ALIGNMENT = 4   /* a device pointer is not 16-byte aligned                       */
 };
@@ -119,7 +119,8 @@ typedef struct GsbRasterArgs {
   float* out_final_T;          /* [H,W]  final transmittance (ImageState.accum_alpha) */
   int32_t* radii;              /* [P]                                               */
   /* num_rendered: int64[4] written asynchronously on `stream` (device or pinned host memory);
-     [0] = instances actually binned, [1] = reference-equivalent count (sum of tile rectangles,
+     [0] = instances the frame bins, i.e. the instances it needs, even when that is more than
+     max_instances, [1] = reference-equivalent count (sum of tile rectangles,
      what rasterize_points.cu:114 returns), [2] = 1 if the frame needed more than max_instances
      (outputs invalid), [3] = 1 if gsb_raster_forward_pair found view depths that differ between the
      eyes (outputs invalid; always 0 for gsb_raster_forward).  May be NULL.                 */
@@ -136,12 +137,12 @@ typedef struct GsbRasterArgs {
 size_t gsb_raster_workspace_bytes(int32_t P, int32_t width, int32_t height, int64_t max_instances);
 
 /* Enqueue one forward pass.  If the frame needs more than args->max_instances pairs the call
- * returns GSB_ERR_WORKSPACE and gsb_raster_required_instances() tells how many are needed
- * (outputs are then undefined).  Without GSB_RASTER_ASYNC the call waits for the stream ONCE, at
- * the end of the frame, to be able to report that; the reference blocks in the middle of the
- * frame instead (rasterizer_impl.cu:281).  With GSB_RASTER_ASYNC nothing waits. */
+ * returns GSB_ERR_WORKSPACE (outputs are then undefined).  Without GSB_RASTER_ASYNC the call waits
+ * for the stream ONCE, at the end of the frame, to be able to report that; the reference blocks in
+ * the middle of the frame instead (rasterizer_impl.cu:281).  With GSB_RASTER_ASYNC nothing waits.
+ * Pass num_rendered to learn how many pairs the frame needs: after GSB_ERR_WORKSPACE its [0] is
+ * already written, because the call waited. */
 int gsb_raster_forward(const GsbRasterArgs* args, void* stream);
-int64_t gsb_raster_required_instances(void);
 
 /* Both eyes of a stereo pair in one call -- what Renderer.render_image_pair (renderer_utils.py:378-389) does with two
  * back-to-back forward calls on the same Gaussian cloud.  The Gaussian parameters are read ONCE (one fused preprocess

@@ -68,7 +68,7 @@ def _np_inputs(g, vt, **over):
     return {k: v for k, v in d.items() if v is not None or k in ()}
 
 
-def _ours(dev, inp, flags=None, **kw):
+def _ours(dev, inp, flags=None, want_counts=True, **kw):
     import torch
 
     from gs2mesh_b200 import rasterizer as rast
@@ -79,7 +79,7 @@ def _ours(dev, inp, flags=None, **kw):
         campos=t(inp["campos"]), bg=t(inp["bg"]), width=inp["W"], height=inp["H"], tan_fovx=inp["tan_fovx"],
         tan_fovy=inp["tan_fovy"], shs=t(inp.get("shs")), colors_precomp=t(inp.get("colors_precomp")), scales=t(inp.get("scales")),
         rotations=t(inp.get("rotations")), cov3D_precomp=t(inp.get("cov3D_precomp")), sh_degree=inp["sh_degree"],
-        scale_modifier=inp["scale_modifier"], flags=rast.DEFAULT_FLAGS if flags is None else flags, want_counts=True, **kw)
+        scale_modifier=inp["scale_modifier"], flags=rast.DEFAULT_FLAGS if flags is None else flags, want_counts=want_counts, **kw)
     torch.cuda.synchronize()
     return {k: (v.cpu().numpy() if v is not None else None) for k, v in out.items()}
 
@@ -339,19 +339,45 @@ def test_edge_sizes(oracle, gsb_lib, cuda_device):
         _assert_parity(ours["final_T"], o["final_T"], f"final_T n={n}", budget=1e-3)
 
 
-def test_workspace_too_small_is_reported(gsb_lib, cuda_device):
+def test_workspace_too_small_reports_need_in_num_rendered(gsb_lib, cuda_device):
     import torch
 
     from gs2mesh_b200 import _lib
 
     g, vt = _case(3000, 320, 240, seed=0)
     for flags in (0, _lib.RASTER_CUB_SORT):
-        rc, _, _ = _raw_call(gsb_lib, cuda_device, g, vt, 1000, flags)
+        status = torch.zeros(4, dtype=torch.int64).pin_memory()
+        rc, _, _ = _raw_call(gsb_lib, cuda_device, g, vt, 1000, flags, status)
         assert rc == _lib.GSB_ERR_WORKSPACE
-        need = gsb_lib.gsb_raster_required_instances()
+        need = int(status[0])  # the call waited, so the frame's need is already written
         assert need > 1000 and b"instances" in gsb_lib.gsb_last_error()
         rc, col, _ = _raw_call(gsb_lib, cuda_device, g, vt, need, flags)
         assert rc == _lib.GSB_OK and torch.isfinite(col).all() and float(col.mean()) > 0.01
+
+
+def test_wrapper_grows_undersized_scratch_and_renders_again(gsb_lib, cuda_device, monkeypatch):
+    """The synchronous wrapper learns the frame's need from the counts buffer it always hands the library, grows the scratch
+    block and renders the frame again inside the call, whether or not the caller asked for the counts."""
+    from gs2mesh_b200 import rasterizer as rast
+
+    g, vt = _case(10000, 640, 480, seed=1)
+    inp = _np_inputs(g, vt)
+    ample = _ours(cuda_device, inp)
+    need = int(ample["counts"][0])
+    assert need > 1024
+    monkeypatch.setattr(rast, "MIN_GUESS", 1024)
+    monkeypatch.setattr(rast, "GUESS_PER_GAUSSIAN", 0)
+    for want_counts in (False, True):
+        monkeypatch.setattr(rast, "_scratch", {})  # the first attempt gets a 1024-instance scratch block
+        got = _ours(cuda_device, inp, want_counts=want_counts)
+        (scratch,) = rast._scratch.values()
+        assert scratch.max_instances >= need  # grown, so the frame was rendered again
+        for k in ("color", "depth", "final_T", "radii"):
+            np.testing.assert_array_equal(got[k], ample[k], err_msg=f"{k} want_counts={want_counts}")
+        if want_counts:
+            np.testing.assert_array_equal(got["counts"], ample["counts"])
+        else:
+            assert got["counts"] is None
 
 
 def test_invalid_argument_combinations(gsb_lib, cuda_device):
