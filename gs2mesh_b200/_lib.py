@@ -77,13 +77,11 @@ SIGNATURES = {
     "gsb_tsdf_touch": (C.c_int, [_vp, _vp, C.c_int32, C.c_int32, C.c_double, C.c_double, C.c_double, C.c_double, C.POINTER(C.c_double), _vp]),
     "gsb_tsdf_to_sums": (C.c_int, [_vp, _vp]),
     "gsb_tsdf_from_sums": (C.c_int, [_vp, _vp]),
-    "gsb_tsdf_sums_bricks": (C.c_int, [_vp, C.c_int, _vp, C.c_uint32, _vp]),
     "gsb_tsdf_find_bricks": (C.c_int, [_vp, _vp, C.c_uint32, C.c_int, _vp, _vp, _vp]),
     "gsb_tsdf_export_dense": (C.c_int, [_vp, C.POINTER(C.c_int32), C.POINTER(C.c_int32), _vp, _vp, _vp]),
     "gsb_tsdf_last_stats": (C.c_int, [_vp, _vp, _vp]),
     "gsb_tsdf_reduce_scratch_bytes": (C.c_size_t, [_vp, C.c_int, C.c_uint32]),
-    "gsb_tsdf_reduce": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_int, _vp, C.c_size_t, _vp]),
-    "gsb_tsdf_reduce_required_bytes": (C.c_size_t, []),
+    "gsb_tsdf_reduce": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_int, _vp, C.c_size_t, C.POINTER(C.c_size_t), _vp]),
     "gsb_comm_unique_id": (C.c_int, [_vp]),
     "gsb_comm_create": (_vp, [_vp, C.c_int, C.c_int]),
     "gsb_comm_destroy": (None, [_vp]),

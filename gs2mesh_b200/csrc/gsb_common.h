@@ -153,6 +153,37 @@ __host__ __device__ inline uint32_t brick_hash(unsigned long long key, uint32_t 
   key ^= key >> 33;
   return (uint32_t)key & mask;
 }
+// counters (uint32[8]): [0] entries queued this frame  [1] bricks dropped this frame (pool full)
+//                       [2] brick-box cells outside the lattice this frame
+//                       [4] pool slots in use (persistent)  [5] bricks dropped since creation (persistent)
+//                       [6] brick-box cells outside the lattice since creation (persistent)
+// Every drop and every out-of-range cell is added to its per-frame word and its persistent word with atomics where it is
+// found, so no kernel folds one into the other.
+constexpr int kCntQueued = 0, kCntDropped = 1, kCntOutOfRange = 2, kCntPool = 4, kCntDroppedTotal = 5, kCntOutOfRangeTotal = 6;
+
+struct HashView {
+  unsigned long long* keys;
+  uint32_t* vals;
+  uint32_t* stamp;
+  int32_t* index;  // [pool][4]
+  uint32_t mask, pool;
+};
+
+inline HashView hash_view(const GsbVolumeDesc& d) {
+  HashView hv;
+  hv.keys = reinterpret_cast<unsigned long long*>(d.hash_keys);
+  hv.vals = d.hash_vals;
+  hv.stamp = d.hash_stamp;
+  hv.index = d.brick_index;
+  hv.mask = d.hash_slots - 1u;
+  hv.pool = d.pool_bricks;
+  return hv;
+}
+
+// sums_pair in place over the pool slots in use among the first `bricks` (gsb_tsdf.cu): gsb_tsdf_to_sums / from_sums over
+// the whole pool, the merge's canonical rank over the union at the front of its pool
+int tsdf_sums(GsbVolume* vol, bool to_sums, uint32_t bricks, cudaStream_t stream);
+
 #ifdef __CUDACC__
 // position of `key` in the table, or kSlotNone
 __device__ inline uint32_t brick_find(const unsigned long long* __restrict__ keys, uint32_t mask, unsigned long long key) {
@@ -163,6 +194,82 @@ __device__ inline uint32_t brick_find(const unsigned long long* __restrict__ key
     if (k == kHashEmpty) return kSlotNone;
   }
   return kSlotNone;
+}
+
+__device__ __forceinline__ void count_dropped(uint32_t* counters) {
+  atomicAdd(&counters[kCntDropped], 1u);
+  atomicAdd(&counters[kCntDroppedTotal], 1u);
+}
+__device__ __forceinline__ void count_out_of_range(uint32_t* counters) {
+  atomicAdd(&counters[kCntOutOfRange], 1u);
+  atomicAdd(&counters[kCntOutOfRangeTotal], 1u);
+}
+
+// position of brick (bx,by,bz) in the table, inserting it (and giving it the next pool slot) if absent; kSlotNone if the
+// brick cannot be stored.  The pool slot of a fresh key is written by the inserting thread with a plain store: readers of
+// hash_vals are always a later kernel.  Threads that pass the pool check together can all insert; those whose slot lands
+// past the pool leave a dead key (hash_vals = kSlotNone) and still return its position.  A dead key is therefore counted
+// as dropped by whoever reads its slot: integrate_kernel, count_dead_kernel (touch), resolve_slots_kernel and
+// insert_gathered_kernel (merge).
+__device__ __forceinline__ uint32_t brick_find_or_insert(const HashView& hv, uint32_t* __restrict__ counters, int bx, int by,
+                                                         int bz) {
+  if (!brick_key_ok(bx, by, bz)) return kSlotNone;
+  const unsigned long long key = brick_key(bx, by, bz);
+  uint32_t h = brick_hash(key, hv.mask);
+  for (uint32_t probe = 0; probe <= hv.mask; ++probe, h = (h + 1) & hv.mask) {
+    unsigned long long k = hv.keys[h];
+    if (k == kHashEmpty) {
+      // pool exhausted: do not grow the table any further (racy by a few entries at most, bounded by the probe limit)
+      if (*(volatile uint32_t*)&counters[kCntPool] >= hv.pool) return kSlotNone;
+      k = atomicCAS(&hv.keys[h], kHashEmpty, key);
+      if (k == kHashEmpty) {  // inserted: OpenVolumeUnit
+        const uint32_t slot = atomicAdd(&counters[kCntPool], 1u);
+        if (slot < hv.pool) {
+          hv.vals[h] = slot;
+          reinterpret_cast<int4*>(hv.index)[slot] = make_int4(bx, by, bz, 0);
+        } else {
+          hv.vals[h] = kSlotNone;
+          atomicSub(&counters[kCntPool], 1u);
+        }
+        return h;
+      }
+    }
+    if (k == key) return h;
+  }
+  return kSlotNone;
+}
+
+// (mean, weight) <-> (sum, weight) of one voxel pair in registers, the one statement of the conversion: v = (tsdf0, w0,
+// tsdf1, w1), c[k] the colour of voxel k (with_color).  to_sums: tsdf*w, rgb*w; else tsdf/w (0 where w is 0), rgb/w.
+// Callers skip a pair whose two weights are 0 (it is not stored back in place), and the colour of a voxel of weight 0 is
+// not converted (callers need not load it).  Skipping gives the bits converting would give, because a voxel of weight 0
+// holds tsdf 0 and colour 0: pools start zero-filled, integrate_kernel writes only the voxels it fuses and fuse_voxel
+// leaves them with weight >= 1, and the merge's from-sums step writes tsdf 0 and a colour of 0 where the summed weight is
+// 0 (a sum of weights >= 0 is 0 only if every rank's weight was, and so were their tsdf and colour).
+__device__ __forceinline__ void sums_pair(float4& v, float4 (&c)[2], bool with_color, bool to_sums) {
+  const float w0 = v.y, w1 = v.w;
+  if (to_sums) {
+    v.x *= w0;
+    v.z *= w1;
+  } else {
+    v.x = w0 > 0.f ? v.x / w0 : 0.f;
+    v.z = w1 > 0.f ? v.z / w1 : 0.f;
+  }
+  if (!with_color) return;
+#pragma unroll
+  for (int k = 0; k < 2; ++k) {
+    const float w = k ? w1 : w0;
+    if (w == 0.f) continue;
+    if (to_sums) {
+      c[k].x *= w;
+      c[k].y *= w;
+      c[k].z *= w;
+    } else {
+      c[k].x /= w;
+      c[k].y /= w;
+      c[k].z /= w;
+    }
+  }
 }
 #endif
 

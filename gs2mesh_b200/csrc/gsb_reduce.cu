@@ -76,43 +76,21 @@ NcclApi& nccl() {
       return ::gsb::fail(GSB_ERR_CUDA, "%s failed: %s (%s:%d)", #expr, nccl().GetErrorString(r__), __FILE__, __LINE__); \
   } while (0)
 
-constexpr int kCntDropped = 1, kCntPool = 4;
-
-// every rank's brick list (gathered: [nranks][pool] int4, counts[nranks]) -> this rank's hash; missing bricks are opened
-__global__ void __launch_bounds__(256) insert_gathered_kernel(unsigned long long* __restrict__ keys, uint32_t* __restrict__ vals,
-                                                              int4* __restrict__ index, uint32_t mask, uint32_t pool,
-                                                              uint32_t* __restrict__ counters, const int4* __restrict__ gathered,
-                                                              const uint32_t* __restrict__ counts, int nranks, int self) {
+// every rank's brick list (gathered: [nranks][pool] int4, counts[nranks]) -> this rank's hash; missing bricks are opened.
+// A brick that cannot be stored counts as dropped: always in the thread that left it without a slot, and in a thread that
+// finds it once its slot is stored (a copy of the brick from another rank may find the key first).
+__global__ void __launch_bounds__(256) insert_gathered_kernel(const HashView hv, uint32_t* __restrict__ counters,
+                                                              const int4* __restrict__ gathered, const uint32_t* __restrict__ counts,
+                                                              int nranks, int self) {
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= (size_t)nranks * pool) return;
-  const int r = (int)(i / pool);
-  const uint32_t j = (uint32_t)(i % pool);
-  if (r == self || j >= min(counts[r], pool)) return;
+  if (i >= (size_t)nranks * hv.pool) return;
+  const int r = (int)(i / hv.pool);
+  const uint32_t j = (uint32_t)(i % hv.pool);
+  if (r == self || j >= min(counts[r], hv.pool)) return;
   const int4 b = gathered[i];
   if (!brick_key_ok(b.x, b.y, b.z)) return;
-  const unsigned long long key = brick_key(b.x, b.y, b.z);
-  uint32_t h = brick_hash(key, mask);
-  for (uint32_t probe = 0; probe <= mask; ++probe, h = (h + 1) & mask) {
-    unsigned long long k = keys[h];
-    if (k == kHashEmpty) {
-      if (*(volatile uint32_t*)&counters[kCntPool] >= pool) break;
-      k = atomicCAS(&keys[h], kHashEmpty, key);
-      if (k == kHashEmpty) {
-        const uint32_t slot = atomicAdd(&counters[kCntPool], 1u);
-        if (slot < pool) {
-          vals[h] = slot;
-          index[slot] = make_int4(b.x, b.y, b.z, 0);
-        } else {
-          vals[h] = kSlotNone;
-          atomicSub(&counters[kCntPool], 1u);
-          atomicAdd(&counters[kCntDropped], 1u);
-        }
-        return;
-      }
-    }
-    if (k == key) return;
-  }
-  atomicAdd(&counters[kCntDropped], 1u);
+  const uint32_t h = brick_find_or_insert(hv, counters, b.x, b.y, b.z);
+  if (h == kSlotNone || hv.vals[h] >= hv.pool) count_dropped(counters);
 }
 
 // canonical order (the canonical rank's brick_index[0 .. n)) -> this rank's pool slots (kSlotNone: this rank never saw it)
@@ -130,104 +108,32 @@ __global__ void __launch_bounds__(256) map_canonical_kernel(const unsigned long 
   slot_of[i] = slot < pool ? slot : kSlotNone;
 }
 
-// pool -> packed payload in canonical order, (mean, w) -> (sum, w) on the way; bricks this rank never saw travel as zeros
-__global__ void __launch_bounds__(256) pack_sums_kernel(const float4* __restrict__ tw, const float4* __restrict__ color,
+// the payload in canonical order <-> the pool, through slot_of (the pool slot of every payload brick): to_sums gathers
+// pool -> payload, where a brick this rank never saw travels as zeros; else scatters payload -> pool, where a brick
+// without a slot (only if this rank's pool was exhausted while opening the union, counted as dropped) is not written.
+// A pair of weight 0 moves as it is and the colour of a voxel of weight 0 as zeros (sums_pair).
+template <bool to_sums>
+__global__ void __launch_bounds__(256) move_sums_kernel(float4* __restrict__ tw, float4* __restrict__ color,
                                                         const uint32_t* __restrict__ slot_of, uint32_t n, float4* __restrict__ ptw,
                                                         float4* __restrict__ pcolor) {
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;  // voxel pair of the payload
   if (i >= (size_t)n * (GSB_BRICK_VOXELS / 2)) return;
   const uint32_t slot = slot_of[i / (GSB_BRICK_VOXELS / 2)];
-  const size_t src = (size_t)slot * (GSB_BRICK_VOXELS / 2) + i % (GSB_BRICK_VOXELS / 2);
+  if (slot == kSlotNone && !to_sums) return;
+  const size_t p = (size_t)slot * (GSB_BRICK_VOXELS / 2) + i % (GSB_BRICK_VOXELS / 2);  // voxel pair of the pool
   float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-  if (slot != kSlotNone) v = tw[src];
-  const float w0 = v.y, w1 = v.w;
-  v.x *= w0;
-  v.z *= w1;
-  ptw[i] = v;
-  if (pcolor) {
-    float4 c0 = make_float4(0.f, 0.f, 0.f, 0.f), c1 = c0;
-    if (slot != kSlotNone && (w0 != 0.f || w1 != 0.f)) {
-      c0 = color[2 * src];
-      c1 = color[2 * src + 1];
-      c0.x *= w0;
-      c0.y *= w0;
-      c0.z *= w0;
-      c1.x *= w1;
-      c1.y *= w1;
-      c1.z *= w1;
-    }
-    pcolor[2 * i] = c0;
-    pcolor[2 * i + 1] = c1;
-  }
-}
-
-// reduced payload -> pool, (sum, w) -> (mean, w)
-__global__ void __launch_bounds__(256) unpack_means_kernel(float4* __restrict__ tw, float4* __restrict__ color,
-                                                           const uint32_t* __restrict__ slot_of, uint32_t n,
-                                                           const float4* __restrict__ ptw, const float4* __restrict__ pcolor) {
-  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= (size_t)n * (GSB_BRICK_VOXELS / 2)) return;
-  const uint32_t slot = slot_of[i / (GSB_BRICK_VOXELS / 2)];
-  if (slot == kSlotNone) return;  // only if this rank's pool was exhausted while opening the union (counted as dropped)
-  const size_t dst = (size_t)slot * (GSB_BRICK_VOXELS / 2) + i % (GSB_BRICK_VOXELS / 2);
-  float4 v = ptw[i];
-  const float w0 = v.y, w1 = v.w;
-  v.x = w0 > 0.f ? v.x / w0 : 0.f;
-  v.z = w1 > 0.f ? v.z / w1 : 0.f;
-  tw[dst] = v;
-  if (color && pcolor) {
-    float4 c0 = pcolor[2 * i], c1 = pcolor[2 * i + 1];
-    if (w0 > 0.f) {
-      c0.x /= w0;
-      c0.y /= w0;
-      c0.z /= w0;
-    }
-    if (w1 > 0.f) {
-      c1.x /= w1;
-      c1.y /= w1;
-      c1.z /= w1;
-    }
-    color[2 * dst] = c0;
-    color[2 * dst + 1] = c1;
-  }
-}
-
-// in-place conversion of the canonical rank's pool prefix [0, n): mode 0 (mean,w)->(sum,w), 1 back
-__global__ void __launch_bounds__(256) prefix_sums_kernel(float4* __restrict__ tw, float4* __restrict__ color, uint32_t n, int mode) {
-  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= (size_t)n * (GSB_BRICK_VOXELS / 2)) return;
-  float4 v = tw[i];
-  if (v.y == 0.f && v.w == 0.f) return;
-  const float w0 = v.y, w1 = v.w;
-  if (mode == 0) {
-    v.x *= w0;
-    v.z *= w1;
-  } else {
-    v.x = w0 > 0.f ? v.x / w0 : 0.f;
-    v.z = w1 > 0.f ? v.z / w1 : 0.f;
-  }
-  tw[i] = v;
-  if (color) {
+  if (slot != kSlotNone) v = to_sums ? tw[p] : ptw[i];
+  float4 c[2] = {make_float4(0.f, 0.f, 0.f, 0.f), make_float4(0.f, 0.f, 0.f, 0.f)};
+  if (color)
 #pragma unroll
-    for (int k = 0; k < 2; ++k) {
-      const float w = k ? w1 : w0;
-      if (w == 0.f) continue;
-      float4 c = color[2 * i + k];
-      if (mode == 0) {
-        c.x *= w;
-        c.y *= w;
-        c.z *= w;
-      } else {
-        c.x /= w;
-        c.y /= w;
-        c.z /= w;
-      }
-      color[2 * i + k] = c;
-    }
-  }
+    for (int k = 0; k < 2; ++k)
+      if ((k ? v.w : v.y) != 0.f) c[k] = to_sums ? color[2 * p + k] : pcolor[2 * i + k];
+  sums_pair(v, c, color != nullptr, to_sums);
+  (to_sums ? ptw[i] : tw[p]) = v;
+  if (color)
+#pragma unroll
+    for (int k = 0; k < 2; ++k) (to_sums ? pcolor[2 * i + k] : color[2 * p + k]) = c[k];
 }
-
-thread_local size_t g_reduce_required = 0;
 
 struct ReduceScratch {
   uint32_t* counts;      // [nranks] pool slots in use on every rank
@@ -301,10 +207,8 @@ size_t gsb_tsdf_reduce_scratch_bytes(const GsbVolume* vol, int nranks, uint32_t 
   return carve_reduce(nullptr, vol->d.pool_bricks, nranks, union_bricks, vol->d.color != nullptr).total;
 }
 
-size_t gsb_tsdf_reduce_required_bytes(void) { return g_reduce_required; }
-
 int gsb_tsdf_reduce(GsbVolume* vol, void* nccl_comm, int nranks, int rank, int root, void* scratch, size_t scratch_bytes,
-                    void* stream_v) {
+                    size_t* required_bytes, void* stream_v) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
   if (!vol || !nccl_comm || nranks <= 0 || rank < 0 || rank >= nranks || root >= nranks || !scratch)
     return fail(GSB_ERR_INVALID, "tsdf_reduce: bad arguments");
@@ -319,7 +223,7 @@ int gsb_tsdf_reduce(GsbVolume* vol, void* nccl_comm, int nranks, int rank, int r
   const bool canonical = rank == canon_rank;
   ReduceScratch rs = carve_reduce(scratch, pool, nranks, 0, with_color);
   if (rs.fixed_bytes > scratch_bytes) {
-    g_reduce_required = carve_reduce(nullptr, pool, nranks, pool / 8 + 1, with_color).total;
+    if (required_bytes) *required_bytes = carve_reduce(nullptr, pool, nranks, pool / 8 + 1, with_color).total;
     return fail(GSB_ERR_WORKSPACE, "tsdf_reduce: scratch has %zu bytes, at least %zu needed", scratch_bytes, rs.fixed_bytes);
   }
   unsigned long long* keys = reinterpret_cast<unsigned long long*>(d.hash_keys);
@@ -327,62 +231,57 @@ int gsb_tsdf_reduce(GsbVolume* vol, void* nccl_comm, int nranks, int rank, int r
   float4* tw = reinterpret_cast<float4*>(d.tsdf_weight);
   float4* color = reinterpret_cast<float4*>(d.color);
 
-  // 1. every rank's brick list
-  StageTimer* tm_index = new StageTimer(kStMergeIndex, stream);
-  struct Guard {  // the timer closes when the index phase ends, on every exit path
-    StageTimer*& t;
-    ~Guard() { delete t; t = nullptr; }
-  } guard{tm_index};
-  GSB_NCCL_OK(nccl().GroupStart());
-  GSB_NCCL_OK(nccl().AllGather(d.counters + kCntPool, rs.counts, 1, ncclUint32, comm, stream));
-  GSB_NCCL_OK(nccl().AllGather(index, rs.gathered, (size_t)pool * 4, ncclInt32, comm, stream));
-  GSB_NCCL_OK(nccl().GroupEnd());
-  // 2. the ranks that receive the result open the bricks they lack
-  if (canonical || all) {
-    const size_t n = (size_t)nranks * pool;
-    insert_gathered_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(keys, d.hash_vals, index, mask, pool, d.counters,
-                                                                            rs.gathered, rs.counts, nranks, rank);
-    count_launch();
-  }
-  // 3. the canonical rank's brick order (its pool order after step 2) is the order of the exchange
-  GSB_NCCL_OK(nccl().GroupStart());
-  GSB_NCCL_OK(nccl().Broadcast(d.counters + kCntPool, rs.n_union, 1, ncclUint32, canon_rank, comm, stream));
-  GSB_NCCL_OK(nccl().Broadcast(index, canonical ? index : rs.canon, (size_t)pool * 4, ncclInt32, canon_rank, comm, stream));
-  GSB_NCCL_OK(nccl().GroupEnd());
   uint32_t n_union = 0;  // the one host read of the merge: NCCL needs the payload size as a count
-  GSB_CUDA_OK(cudaMemcpyAsync(&n_union, rs.n_union, sizeof(uint32_t), cudaMemcpyDeviceToHost, stream));
-  GSB_CUDA_OK(cudaStreamSynchronize(stream));
-  delete tm_index;
-  tm_index = nullptr;
+  {
+    StageTimer tm(kStMergeIndex, stream);
+    // 1. every rank's brick list
+    GSB_NCCL_OK(nccl().GroupStart());
+    GSB_NCCL_OK(nccl().AllGather(d.counters + kCntPool, rs.counts, 1, ncclUint32, comm, stream));
+    GSB_NCCL_OK(nccl().AllGather(index, rs.gathered, (size_t)pool * 4, ncclInt32, comm, stream));
+    GSB_NCCL_OK(nccl().GroupEnd());
+    // 2. the ranks that receive the result open the bricks they lack
+    if (canonical || all) {
+      insert_gathered_kernel<<<blocks_for((long long)nranks * pool), 256, 0, stream>>>(hash_view(d), d.counters, rs.gathered,
+                                                                                     rs.counts, nranks, rank);
+      count_launch();
+    }
+    // 3. the canonical rank's brick order (its pool order after step 2) is the order of the exchange
+    GSB_NCCL_OK(nccl().GroupStart());
+    GSB_NCCL_OK(nccl().Broadcast(d.counters + kCntPool, rs.n_union, 1, ncclUint32, canon_rank, comm, stream));
+    GSB_NCCL_OK(nccl().Broadcast(index, canonical ? index : rs.canon, (size_t)pool * 4, ncclInt32, canon_rank, comm, stream));
+    GSB_NCCL_OK(nccl().GroupEnd());
+    GSB_CUDA_OK(cudaMemcpyAsync(&n_union, rs.n_union, sizeof(uint32_t), cudaMemcpyDeviceToHost, stream));
+    GSB_CUDA_OK(cudaStreamSynchronize(stream));
+  }
   if (n_union > pool) n_union = pool;
   if (n_union == 0) return GSB_OK;
   rs = carve_reduce(scratch, pool, nranks, canonical ? 0 : n_union, with_color);
-  g_reduce_required = carve_reduce(nullptr, pool, nranks, n_union, with_color).total;  // same on every rank
-  if (g_reduce_required > scratch_bytes)
-    return fail(GSB_ERR_WORKSPACE, "tsdf_reduce: scratch has %zu bytes, %zu needed for %u bricks", scratch_bytes, g_reduce_required,
-                n_union);
+  const size_t need = carve_reduce(nullptr, pool, nranks, n_union, with_color).total;  // same on every rank
+  if (need > scratch_bytes) {
+    if (required_bytes) *required_bytes = need;
+    return fail(GSB_ERR_WORKSPACE, "tsdf_reduce: scratch has %zu bytes, %zu needed for %u bricks", scratch_bytes, need, n_union);
+  }
   const size_t pairs = (size_t)n_union * (GSB_BRICK_VOXELS / 2);
   const unsigned pgrid = (unsigned)((pairs + 255) / 256);
   const float* send_tw;
   const float* send_color = nullptr;
   float* recv_tw;
   float* recv_color = nullptr;
+  int rc;
   {
     StageTimer tm(kStMergePack, stream);
     if (canonical) {  // the pool prefix [0, n_union) IS the payload: convert and exchange it in place
-      prefix_sums_kernel<<<pgrid, 256, 0, stream>>>(tw, color, n_union, 0);
-      count_launch();
+      if ((rc = tsdf_sums(vol, true, n_union, stream))) return rc;
       send_tw = recv_tw = d.tsdf_weight;
       send_color = recv_color = d.color;
     } else {
       map_canonical_kernel<<<(n_union + 255) / 256, 256, 0, stream>>>(keys, d.hash_vals, mask, pool, rs.canon, rs.n_union, rs.slot_of);
-      pack_sums_kernel<<<pgrid, 256, 0, stream>>>(tw, color, rs.slot_of, n_union, rs.ptw, rs.pcolor);
+      move_sums_kernel<true><<<pgrid, 256, 0, stream>>>(tw, color, rs.slot_of, n_union, rs.ptw, rs.pcolor);
       count_launch(2);
       send_tw = recv_tw = reinterpret_cast<float*>(rs.ptw);
       send_color = recv_color = reinterpret_cast<float*>(rs.pcolor);
     }
   }
-  int rc;
   if ((rc = check_launch("tsdf_reduce pack", stream, false))) return rc;
   // 5. ONE reduce of the payload (two buffers in one NCCL group)
   {
@@ -401,10 +300,9 @@ int gsb_tsdf_reduce(GsbVolume* vol, void* nccl_comm, int nranks, int rank, int r
   {
     StageTimer tm(kStMergeUnpack, stream);
     if (canonical) {
-      prefix_sums_kernel<<<pgrid, 256, 0, stream>>>(tw, color, n_union, 1);
-      count_launch();
+      if ((rc = tsdf_sums(vol, false, n_union, stream))) return rc;
     } else if (all) {
-      unpack_means_kernel<<<pgrid, 256, 0, stream>>>(tw, color, rs.slot_of, n_union, rs.ptw, rs.pcolor);
+      move_sums_kernel<false><<<pgrid, 256, 0, stream>>>(tw, color, rs.slot_of, n_union, rs.ptw, rs.pcolor);
       count_launch();
     }
   }

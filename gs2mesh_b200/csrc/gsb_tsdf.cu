@@ -26,64 +26,6 @@
 namespace gsb {
 namespace {
 
-// counters (uint32[8]): [0] entries queued this frame  [1] bricks dropped this frame (pool full)
-//                       [2] brick-box cells outside the lattice this frame
-//                       [4] pool slots in use (persistent)  [5] bricks dropped since creation (persistent)
-//                       [6] brick-box cells outside the lattice since creation (persistent)
-// Every drop and every out-of-range cell is added to its per-frame word and its persistent word with atomics where it is
-// found, so no kernel folds one into the other.
-constexpr int kCntQueued = 0, kCntDropped = 1, kCntOutOfRange = 2, kCntPool = 4, kCntDroppedTotal = 5, kCntOutOfRangeTotal = 6;
-
-__device__ __forceinline__ void count_dropped(uint32_t* counters) {
-  atomicAdd(&counters[kCntDropped], 1u);
-  atomicAdd(&counters[kCntDroppedTotal], 1u);
-}
-__device__ __forceinline__ void count_out_of_range(uint32_t* counters) {
-  atomicAdd(&counters[kCntOutOfRange], 1u);
-  atomicAdd(&counters[kCntOutOfRangeTotal], 1u);
-}
-
-struct HashView {
-  unsigned long long* keys;
-  uint32_t* vals;
-  uint32_t* stamp;
-  int32_t* index;  // [pool][4]
-  uint32_t mask, pool;
-};
-
-// position of brick (bx,by,bz) in the table, inserting it (and giving it the next pool slot) if absent; kSlotNone if the
-// brick cannot be stored.  The pool slot of a fresh key is written by the inserting thread with a plain store: readers of
-// hash_vals are always a later kernel.  Threads that pass the pool check together can all insert; those whose slot lands
-// past the pool leave a dead key (hash_vals = kSlotNone) and still return its position.  A dead key is therefore counted
-// as dropped by whoever reads its slot: integrate_kernel, count_dead_kernel (touch) and resolve_slots_kernel.
-__device__ __forceinline__ uint32_t brick_find_or_insert(const HashView& hv, uint32_t* __restrict__ counters, int bx, int by,
-                                                         int bz) {
-  if (!brick_key_ok(bx, by, bz)) return kSlotNone;
-  const unsigned long long key = brick_key(bx, by, bz);
-  uint32_t h = brick_hash(key, hv.mask);
-  for (uint32_t probe = 0; probe <= hv.mask; ++probe, h = (h + 1) & hv.mask) {
-    unsigned long long k = hv.keys[h];
-    if (k == kHashEmpty) {
-      // pool exhausted: do not grow the table any further (racy by a few entries at most, bounded by the probe limit)
-      if (*(volatile uint32_t*)&counters[kCntPool] >= hv.pool) return kSlotNone;
-      k = atomicCAS(&hv.keys[h], kHashEmpty, key);
-      if (k == kHashEmpty) {  // inserted: OpenVolumeUnit
-        const uint32_t slot = atomicAdd(&counters[kCntPool], 1u);
-        if (slot < hv.pool) {
-          hv.vals[h] = slot;
-          reinterpret_cast<int4*>(hv.index)[slot] = make_int4(bx, by, bz, 0);
-        } else {
-          hv.vals[h] = kSlotNone;
-          atomicSub(&counters[kCntPool], 1u);
-        }
-        return h;
-      }
-    }
-    if (k == key) return h;
-  }
-  return kSlotNone;
-}
-
 struct MarkParams {
   int W, H, nsx, nsy;
   double fx, fy, cx, cy;
@@ -440,45 +382,24 @@ __global__ void __launch_bounds__(256) morph_kernel(const uint8_t* __restrict__ 
   }
 }
 
-// (mean, weight) <-> (sum, weight); mode 0: to sums, 1: from sums.  `bricks` == NULL: every pool slot in use,
-// else only the listed slots (one CTA-row of 2048 voxel pairs per brick).
-__global__ void __launch_bounds__(256) sums_kernel(float4* __restrict__ tw, float4* __restrict__ color, size_t n_pairs, int mode,
-                                                   const uint32_t* __restrict__ bricks, const uint32_t* __restrict__ counters) {
-  size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n_pairs) return;
-  if (bricks != nullptr)
-    i = (size_t)bricks[i / (GSB_BRICK_VOXELS / 2)] * (GSB_BRICK_VOXELS / 2) + i % (GSB_BRICK_VOXELS / 2);
-  else if (i / (GSB_BRICK_VOXELS / 2) >= counters[kCntPool])
-    return;
+// sums_pair in place over the voxel pairs [0, n_pairs) of the pool slots in use
+__global__ void __launch_bounds__(256) sums_kernel(float4* __restrict__ tw, float4* __restrict__ color, size_t n_pairs, int to_sums,
+                                                   const uint32_t* __restrict__ counters) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n_pairs || i / (GSB_BRICK_VOXELS / 2) >= counters[kCntPool]) return;
   float4 v = tw[i];
   if (v.y == 0.f && v.w == 0.f) return;
-  const float w0 = v.y, w1 = v.w;
-  if (mode == 0) {
-    v.x *= w0;
-    v.z *= w1;
-  } else {
-    v.x = w0 > 0.f ? v.x / w0 : 0.f;
-    v.z = w1 > 0.f ? v.z / w1 : 0.f;
-  }
-  tw[i] = v;
-  if (color) {
+  float4 c[2];
+  if (color)
 #pragma unroll
-    for (int k = 0; k < 2; ++k) {
-      const float w = k ? w1 : w0;
-      if (w == 0.f) continue;
-      float4 c = color[2 * i + k];
-      if (mode == 0) {
-        c.x *= w;
-        c.y *= w;
-        c.z *= w;
-      } else {
-        c.x /= w;
-        c.y /= w;
-        c.z /= w;
-      }
-      color[2 * i + k] = c;
-    }
-  }
+    for (int k = 0; k < 2; ++k)
+      if ((k ? v.w : v.y) != 0.f) c[k] = color[2 * i + k];
+  sums_pair(v, c, color != nullptr, to_sums);
+  tw[i] = v;
+  if (color)
+#pragma unroll
+    for (int k = 0; k < 2; ++k)
+      if ((k ? v.w : v.y) != 0.f) color[2 * i + k] = c[k];
 }
 
 // Window of the lattice -> dense x*NY*NZ + y*NZ + z grids (Open3D UniformTSDFVolume indexing); unallocated bricks read as 0.
@@ -596,22 +517,23 @@ int num_sms() {
 }
 
 }  // namespace
+
+int tsdf_sums(GsbVolume* vol, bool to_sums, uint32_t bricks, cudaStream_t stream) {
+  if (!vol) return fail(GSB_ERR_INVALID, "tsdf: volume is NULL");
+  const size_t n_pairs = (size_t)(bricks < vol->d.pool_bricks ? bricks : vol->d.pool_bricks) * (GSB_BRICK_VOXELS / 2);
+  if (n_pairs == 0) return GSB_OK;
+  sums_kernel<<<(unsigned)((n_pairs + 255) / 256), 256, 0, stream>>>(reinterpret_cast<float4*>(vol->d.tsdf_weight),
+                                                                     reinterpret_cast<float4*>(vol->d.color), n_pairs, to_sums,
+                                                                     vol->d.counters);
+  count_launch();
+  return check_launch("sums_kernel", stream, false);
+}
+
 }  // namespace gsb
 
 using namespace gsb;
 
 extern "C" {
-
-static HashView hash_view(const GsbVolumeDesc& d) {
-  HashView hv;
-  hv.keys = reinterpret_cast<unsigned long long*>(d.hash_keys);
-  hv.vals = d.hash_vals;
-  hv.stamp = d.hash_stamp;
-  hv.index = d.brick_index;
-  hv.mask = d.hash_slots - 1u;
-  hv.pool = d.pool_bricks;
-  return hv;
-}
 
 GsbVolume* gsb_tsdf_create(const GsbVolumeDesc* desc) {
   if (!desc || !desc->tsdf_weight || !desc->brick_index || !desc->hash_keys || !desc->hash_vals || !desc->hash_stamp ||
@@ -766,23 +688,8 @@ int gsb_tsdf_integrate(GsbVolume* vol, const float* depth, const uint8_t* rgb, i
   return check_launch("integrate_kernel", stream, false);
 }
 
-static int run_sums(GsbVolume* vol, int mode, const uint32_t* bricks, uint32_t n_bricks, cudaStream_t stream) {
-  if (!vol) return fail(GSB_ERR_INVALID, "tsdf: volume is NULL");
-  const size_t n_pairs = (bricks ? (size_t)n_bricks : (size_t)vol->d.pool_bricks) * (GSB_BRICK_VOXELS / 2);
-  if (n_pairs == 0) return GSB_OK;
-  sums_kernel<<<(unsigned)((n_pairs + 255) / 256), 256, 0, stream>>>(reinterpret_cast<float4*>(vol->d.tsdf_weight),
-                                                                     reinterpret_cast<float4*>(vol->d.color), n_pairs, mode, bricks,
-                                                                     vol->d.counters);
-  count_launch();
-  return check_launch("sums_kernel", stream, false);
-}
-
-int gsb_tsdf_to_sums(GsbVolume* vol, void* stream) { return run_sums(vol, 0, nullptr, 0, static_cast<cudaStream_t>(stream)); }
-int gsb_tsdf_from_sums(GsbVolume* vol, void* stream) { return run_sums(vol, 1, nullptr, 0, static_cast<cudaStream_t>(stream)); }
-int gsb_tsdf_sums_bricks(GsbVolume* vol, int to_sums, const uint32_t* bricks, uint32_t n_bricks, void* stream) {
-  if (n_bricks && !bricks) return fail(GSB_ERR_INVALID, "tsdf_sums_bricks: brick list is NULL");
-  return run_sums(vol, to_sums ? 0 : 1, bricks, n_bricks, static_cast<cudaStream_t>(stream));
-}
+int gsb_tsdf_to_sums(GsbVolume* vol, void* stream) { return tsdf_sums(vol, true, UINT32_MAX, static_cast<cudaStream_t>(stream)); }
+int gsb_tsdf_from_sums(GsbVolume* vol, void* stream) { return tsdf_sums(vol, false, UINT32_MAX, static_cast<cudaStream_t>(stream)); }
 
 int gsb_tsdf_export_dense(const GsbVolume* vol, const int32_t* brick_origin, const int32_t* brick_count, float* tsdf, float* weight,
                           void* stream_v) {

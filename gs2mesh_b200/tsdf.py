@@ -365,15 +365,16 @@ class TSDFVolume:
             # "too small, retry" exit of gsb_tsdf_reduce alone -- and allocated once, so no merge pays for an allocation or for
             # a repeated index exchange (an undersized first guess cost 1.75 ms instead of ~1 ms on 8 GPUs, 61 ms on C4)
             need = int(self._L.gsb_tsdf_reduce_scratch_bytes(self._h, world, self.pool_bricks))
+            required = C.c_size_t(0)
             for _ in range(3):
                 if self._reduce_scratch is None or self._reduce_scratch.numel() < need:
                     self._reduce_scratch = None
                     self._reduce_scratch = torch.empty(need, dtype=torch.uint8, device=self.device)
                 rc = self._L.gsb_tsdf_reduce(self._h, comm, world, rank, -1 if dst is None else int(dst), ptr(self._reduce_scratch),
-                                             self._reduce_scratch.numel(), self._stream())
+                                             self._reduce_scratch.numel(), C.byref(required), self._stream())
                 if rc != _lib.GSB_ERR_WORKSPACE:
                     break
-                need = int(self._L.gsb_tsdf_reduce_required_bytes())  # the same on every rank: all ranks retry together
+                need = required.value  # the same on every rank: all ranks retry together
             _lib.check(rc)
 
 

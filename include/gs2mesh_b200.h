@@ -244,11 +244,10 @@ int gsb_tsdf_integrate(GsbVolume* vol, const float* depth, const uint8_t* rgb, i
 int gsb_tsdf_touch(GsbVolume* vol, const float* depth, int32_t width, int32_t height, double fx, double fy, double cx, double cy,
                    const double* extrinsic_w2c, void* stream);
 
-/* (mean, weight) <-> (sum, weight) of every pool slot in use / of the listed pool slots (device uint32[n_bricks]);
- * to_sums != 0: (mean,w) -> (sum,w).  Building blocks of the cross-rank merge below. */
+/* (mean, weight) -> (sum, weight) / back, in place, of every pool slot in use: (tsdf*w, w, rgb*w) / (tsdf/w, w, rgb/w).
+ * The cross-rank merge below converts with the same arithmetic. */
 int gsb_tsdf_to_sums(GsbVolume* vol, void* stream);
 int gsb_tsdf_from_sums(GsbVolume* vol, void* stream);
-int gsb_tsdf_sums_bricks(GsbVolume* vol, int to_sums, const uint32_t* bricks, uint32_t n_bricks, void* stream);
 
 /* Lattice indices (device int32[n*4]: bx,by,bz,unused) -> pool slots (device uint32[n]; 0xFFFFFFFF = not in the volume).
  * insert != 0 opens missing bricks (zero-filled) like a touch by integrate would.  `scratch` = device uint32[n]. */
@@ -270,7 +269,7 @@ int gsb_tsdf_last_stats(const GsbVolume* vol, uint32_t* out, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Multi-GPU merge of view-sharded volumes (SURVEY.md 8(b) seam 2, 8(e)): ONE call per rank,
- *     gsb_tsdf_reduce(vol, comm, root, scratch, scratch_bytes, stream)
+ *     gsb_tsdf_reduce(vol, comm, nranks, rank, root, scratch, scratch_bytes, &required_bytes, stream)
  * enqueues, on `stream`,
  *   1. an ncclAllGather of every rank's brick lattice indices (fixed-size message, no host round trip),
  *   2. the insertion of the other ranks' bricks into this rank's hash (the receiving ranks open them zero-filled),
@@ -283,14 +282,14 @@ int gsb_tsdf_last_stats(const GsbVolume* vol, uint32_t* out, void* stream);
  * (the libnccl.so.2 torch already loaded), the library does not link against it.
  * scratch: device, >= gsb_tsdf_reduce_scratch_bytes(vol, nranks, bricks in the union) bytes. */
 size_t gsb_tsdf_reduce_scratch_bytes(const GsbVolume* vol, int nranks, uint32_t union_bricks);
-/* Returns GSB_ERR_WORKSPACE when `scratch` cannot hold the packed union (known only after the index exchange);
- * gsb_tsdf_reduce_required_bytes() then tells the size to retry with.  The required size is the same on every rank, so
+/* Returns GSB_ERR_WORKSPACE when `scratch` cannot hold the packed union (known only after the index exchange); it has then
+ * written the size to retry with to *required_bytes (host; may be NULL).  The required size is the same on every rank, so
  * ranks that pass equally sized scratch blocks take the same decision (a collective must not be entered by some ranks
  * only); a retry repeats the cheap index exchange.  root >= 0: ncclReduce to `root` (only its volume is changed);
- * root < 0: ncclAllReduce (every rank ends with the merged volume). */
+ * root < 0: ncclAllReduce (every rank ends with the merged volume).  Bricks a receiving rank's pool cannot hold are
+ * dropped and counted like an integrate's (counters[1] / [5]). */
 int gsb_tsdf_reduce(GsbVolume* vol, void* nccl_comm, int nranks, int rank, int root, void* scratch, size_t scratch_bytes,
-                    void* stream);
-size_t gsb_tsdf_reduce_required_bytes(void);
+                    size_t* required_bytes, void* stream);
 /* Communicator helpers (thin wrappers of ncclGetUniqueId / ncclCommInitRank / ncclCommDestroy): rank 0 creates the
  * 128-byte id, distributes it by any means (torch.distributed broadcast in gs2mesh_b200/tsdf.py), every rank calls
  * gsb_comm_create with it; returns the ncclComm_t as an opaque pointer (NULL on failure, see gsb_last_error). */

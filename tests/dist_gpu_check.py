@@ -3,6 +3,7 @@ view-sharded integration + ONE NCCL sum-reduce of the brick volume == sequential
 
     python -m torch.distributed.run --nnodes=1 --nproc-per-node 2 --master-addr 127.0.0.1 --master-port 29511 tests/dist_gpu_check.py
 """
+import ctypes
 import os
 import sys
 
@@ -36,8 +37,8 @@ def main():
     r = Renderer.from_scene(rigs, baseline, cloud, args=A(), device=f"cuda:{local}")
     r.prepare_renderer()
 
-    def fuse(views):
-        st = TSDF(r, None, A(), "d", window_resolution=128, device=f"cuda:{local}")
+    def fuse(views, pool_bricks=None):
+        st = TSDF(r, None, A(), "d", window_resolution=128, device=f"cuda:{local}", pool_bricks=pool_bricks)
         st.volume = st._make_volume()
         for i in views:
             out = r.render_image_pair(i, to_host=False)
@@ -66,6 +67,7 @@ def main():
     vol.reduce_across_ranks(dst=None)
     torch.cuda.synchronize()
     n, nvox, err, cerr = compare(vol, seq, f"all-reduce on rank {rank}")
+    assert vol.pool_stats()["dropped_total"] == 0, f"all-reduce on rank {rank} dropped bricks"
     # (2) reduce to the last rank: only its volume changes.  First with a scratch that holds the index exchange but no payload:
     #     every rank must get GSB_ERR_WORKSPACE together, with the same required size (the workspace protocol of the C ABI)
     from gs2mesh_b200 import _lib
@@ -75,9 +77,11 @@ def main():
     before = vol2.export_units()
     comm = vol2._comm(None)
     small = torch.empty(int(vol2._L.gsb_tsdf_reduce_scratch_bytes(vol2._h, world, 0)), dtype=torch.uint8, device=vol2.device)
-    rc = vol2._L.gsb_tsdf_reduce(vol2._h, comm, world, rank, root, _lib.ptr(small), small.numel(), vol2._stream())
+    required = ctypes.c_size_t(0)
+    rc = vol2._L.gsb_tsdf_reduce(vol2._h, comm, world, rank, root, _lib.ptr(small), small.numel(), ctypes.byref(required),
+                                 vol2._stream())
     assert rc == _lib.GSB_ERR_WORKSPACE, rc
-    need = torch.tensor([int(vol2._L.gsb_tsdf_reduce_required_bytes())], dtype=torch.int64, device=vol2.device)
+    need = torch.tensor([required.value], dtype=torch.int64, device=vol2.device)
     lo, hi = need.clone(), need.clone()
     dist.all_reduce(lo, op=dist.ReduceOp.MIN)
     dist.all_reduce(hi, op=dist.ReduceOp.MAX)
@@ -89,7 +93,17 @@ def main():
     else:
         after = vol2.export_units()
         assert set(after) == set(before) and all(np.array_equal(after[k][0], before[k][0]) for k in before), "a non-root volume changed"
-    # (3) merging twice in a row with different shards stays consistent: fuse more views into the merged volume
+    assert vol2.pool_stats()["dropped_total"] == 0, f"reduce to root: rank {rank} dropped bricks"
+    # (3) every rank's pool holds its own bricks but not the union: the all-reduce drops the bricks that find no room, and
+    #     counts them where the volume reports its drops
+    most = torch.tensor([own], dtype=torch.int64, device=vol.device)
+    dist.all_reduce(most, op=dist.ReduceOp.MAX)
+    assert n > int(most), "the test needs a union larger than every rank's own bricks"
+    vol3 = fuse(mine, pool_bricks=int(most))
+    assert vol3.pool_stats()["dropped_total"] == 0
+    vol3.reduce_across_ranks(dst=None)
+    torch.cuda.synchronize()
+    assert vol3.num_bricks() == int(most) and vol3.pool_stats()["dropped_total"] > 0, (rank, vol3.pool_stats())
     dist.barrier()
     if rank == 0:
         print(f"dist_gpu_check ok: world={world} views/rank={[len(shard_views(NV, q, world)) for q in range(world)]} "

@@ -33,7 +33,7 @@ def test_version_and_host_only_queries(gsb_lib):
     assert big >= 1_000_000 * 52 + 8_000_000 * 24
 
 
-def test_argument_validation_without_gpu(gsb_lib):
+def test_argument_validation_without_gpu_reduce_reports_need(gsb_lib):
     import ctypes as C
 
     assert gsb_lib.gsb_raster_forward(None, None) == _lib.GSB_ERR_INVALID
@@ -52,7 +52,11 @@ def test_argument_validation_without_gpu(gsb_lib):
     h = gsb_lib.gsb_tsdf_create(C.byref(d))
     assert h is not None
     assert gsb_lib.gsb_tsdf_reduce_scratch_bytes(h, 8, 1000) > 1000 * 4096 * 8  # (sum, w) payload of the union, no colour
-    assert gsb_lib.gsb_tsdf_reduce(h, None, 8, 0, 0, None, 0, None) == _lib.GSB_ERR_INVALID
+    assert gsb_lib.gsb_tsdf_reduce(h, None, 8, 0, 0, None, 0, None, None) == _lib.GSB_ERR_INVALID
+    # the scratch need is written only with GSB_ERR_WORKSPACE: a refused call leaves it as it was
+    need = C.c_size_t(7)
+    assert gsb_lib.gsb_tsdf_reduce(h, None, 8, 0, 0, None, 0, C.byref(need), None) == _lib.GSB_ERR_INVALID
+    assert need.value == 7
     gsb_lib.gsb_tsdf_destroy(h)
 
 
