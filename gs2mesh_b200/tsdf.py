@@ -353,17 +353,31 @@ class TSDFVolume:
         """Merge view-sharded volumes with ONE `gsb_tsdf_reduce` call per rank (include/gs2mesh_b200.h): the ranks exchange
         their brick lattice indices, agree on the union, and sum-reduce (sum tsdf*w, w, sum rgb*w) of exactly those bricks in
         one NCCL reduce (dst = rank) or all-reduce (dst=None); everything runs on the current stream, the only host
-        synchronisation is the read of the union's size.  The root exchanges its pool in place."""
+        synchronisation is the read of the union's size.  The root exchanges its pool in place.
+        A rank whose pool is smaller than another's grows to the largest first; volumes that disagree on `with_color` raise
+        ValueError on every rank."""
         import torch.distributed as dist
 
         if not dist.is_initialized() or dist.get_world_size(group) == 1:
             return
         world, rank = dist.get_world_size(group), dist.get_rank(group)
+        # gsb_tsdf_reduce needs the same pool size, colour setting and scratch size on every rank, but each rank grows its
+        # pool on its own while it integrates: agree on the largest pool (grow keeps every brick) and check the colour
+        agree = torch.tensor([self.pool_bricks, int(self.with_color), 1 - int(self.with_color)], dtype=torch.int64,
+                             device=self.device)
+        dist.all_reduce(agree, op=dist.ReduceOp.MAX, group=group)
+        pool, some_color, some_plain = (int(v) for v in agree.tolist())
+        if some_color and some_plain:
+            raise ValueError("reduce_across_ranks: the ranks' volumes disagree on with_color; all of them must keep colour, "
+                             "or none")
+        if pool > self.pool_bricks:
+            self.grow(pool)
         comm = self._comm(group)
         with torch.cuda.device(self.device):
             # scratch for the worst case (the union fills the pool): the same size on every rank -- a rank must never take the
-            # "too small, retry" exit of gsb_tsdf_reduce alone -- and allocated once, so no merge pays for an allocation or for
-            # a repeated index exchange (an undersized first guess cost 1.75 ms instead of ~1 ms on 8 GPUs, 61 ms on C4)
+            # "too small, retry" exit of gsb_tsdf_reduce alone, so the size passed is `need`, not what an earlier merge left
+            # allocated -- and allocated once, so no merge pays for an allocation or for a repeated index exchange (an
+            # undersized first guess cost 1.75 ms instead of ~1 ms on 8 GPUs, 61 ms on C4)
             need = int(self._L.gsb_tsdf_reduce_scratch_bytes(self._h, world, self.pool_bricks))
             required = C.c_size_t(0)
             for _ in range(3):
@@ -371,7 +385,7 @@ class TSDFVolume:
                     self._reduce_scratch = None
                     self._reduce_scratch = torch.empty(need, dtype=torch.uint8, device=self.device)
                 rc = self._L.gsb_tsdf_reduce(self._h, comm, world, rank, -1 if dst is None else int(dst), ptr(self._reduce_scratch),
-                                             self._reduce_scratch.numel(), C.byref(required), self._stream())
+                                             need, C.byref(required), self._stream())
                 if rc != _lib.GSB_ERR_WORKSPACE:
                     break
                 need = required.value  # the same on every rank: all ranks retry together

@@ -287,7 +287,13 @@ size_t gsb_tsdf_reduce_scratch_bytes(const GsbVolume* vol, int nranks, uint32_t 
  * ranks that pass equally sized scratch blocks take the same decision (a collective must not be entered by some ranks
  * only); a retry repeats the cheap index exchange.  root >= 0: ncclReduce to `root` (only its volume is changed);
  * root < 0: ncclAllReduce (every rank ends with the merged volume).  Bricks a receiving rank's pool cannot hold are
- * dropped and counted like an integrate's (counters[1] / [5]). */
+ * dropped and counted like an integrate's (counters[1] / [5]).
+ * Precondition: every rank passes a volume with the same pool_bricks and the same colour setting (colour on every rank or
+ * on none), and the same scratch_bytes; the element counts of the collectives are derived from them, so ranks that differ
+ * enter mismatched collectives.  TSDFVolume.reduce_across_ranks agrees on them before the call.
+ * A GSB_ERR_WORKSPACE returned after the index exchange (scratch holds the fixed part but not the payload) leaves the
+ * union's bricks opened, zero-filled, on the receiving ranks; a retry finds them and gives the bits a first call with
+ * enough scratch gives. */
 int gsb_tsdf_reduce(GsbVolume* vol, void* nccl_comm, int nranks, int rank, int root, void* scratch, size_t scratch_bytes,
                     size_t* required_bytes, void* stream);
 /* Communicator helpers (thin wrappers of ncclGetUniqueId / ncclCommInitRank / ncclCommDestroy): rank 0 creates the
