@@ -374,22 +374,17 @@ class TSDFVolume:
             self.grow(pool)
         comm = self._comm(group)
         with torch.cuda.device(self.device):
-            # scratch for the worst case (the union fills the pool): the same size on every rank -- a rank must never take the
-            # "too small, retry" exit of gsb_tsdf_reduce alone, so the size passed is `need`, not what an earlier merge left
-            # allocated -- and allocated once, so no merge pays for an allocation or for a repeated index exchange (an
-            # undersized first guess cost 1.75 ms instead of ~1 ms on 8 GPUs, 61 ms on C4)
+            # scratch for a union that fills the pool, the most gsb_tsdf_reduce can need (it clamps the union to the pool), so
+            # it never returns GSB_ERR_WORKSPACE here; the same size on every rank, since every rank now has the same pool.  The
+            # size passed is `need`, not what an earlier merge left allocated.  Allocated once, so no merge pays for an
+            # allocation or for a repeated index exchange (an undersized first guess cost 1.75 ms instead of ~1 ms on 8 GPUs,
+            # 61 ms on C4; measured once, script since removed)
             need = int(self._L.gsb_tsdf_reduce_scratch_bytes(self._h, world, self.pool_bricks))
-            required = C.c_size_t(0)
-            for _ in range(3):
-                if self._reduce_scratch is None or self._reduce_scratch.numel() < need:
-                    self._reduce_scratch = None
-                    self._reduce_scratch = torch.empty(need, dtype=torch.uint8, device=self.device)
-                rc = self._L.gsb_tsdf_reduce(self._h, comm, world, rank, -1 if dst is None else int(dst), ptr(self._reduce_scratch),
-                                             need, C.byref(required), self._stream())
-                if rc != _lib.GSB_ERR_WORKSPACE:
-                    break
-                need = required.value  # the same on every rank: all ranks retry together
-            _lib.check(rc)
+            if self._reduce_scratch is None or self._reduce_scratch.numel() < need:
+                self._reduce_scratch = None
+                self._reduce_scratch = torch.empty(need, dtype=torch.uint8, device=self.device)
+            _lib.check(self._L.gsb_tsdf_reduce(self._h, comm, world, rank, -1 if dst is None else int(dst),
+                                               ptr(self._reduce_scratch), need, None, self._stream()))
 
 
 def filter_object_mask(mask, closing_kernel_size: int = 10, erosion_kernel_size: int = 10, invert: bool = False, device="cuda"):
@@ -411,80 +406,6 @@ def filter_object_mask(mask, closing_kernel_size: int = 10, erosion_kernel_size:
             _lib.check(L.gsb_mask_morphology(ptr(a), w, h, int(k), dilate, ptr(b), stream))
             a, b = b, a
     return a
-
-
-def merge_units_protocol(units, group=None, dst: Optional[int] = None, pool_bricks: int = 4096):
-    """Host-side statement of `gsb_tsdf_reduce`'s protocol (csrc/gsb_reduce.cu), step for step, on numpy units
-    {(bx,by,bz): tsdf_weight float32 [4096,2]} with torch.distributed collectives of ANY backend -- what the CPU (gloo,
-    world_size 2) tests run, since the device path needs GPUs:
-      1. all-gather of every rank's (count, fixed-size padded list of brick lattice indices);
-      2. the receiving ranks open the bricks they lack (zero-filled);
-      3. broadcast of the canonical rank's brick order;
-      4. pack in canonical order, (mean,w) -> (sum,w), bricks a rank never saw travel as zeros;
-      5. ONE sum reduce (dst) / all-reduce (dst=None) of the packed payload;
-      6. (sum,w) -> (mean,w) where the result lives.
-    Returns this rank's units after the merge."""
-    import torch.distributed as dist
-
-    world, rank = dist.get_world_size(group), dist.get_rank(group)
-    canon_rank = 0 if dst is None else int(dst)
-    receives = dst is None or rank == canon_rank
-    units = {k: np.array(v, dtype=np.float32, copy=True) for k, v in units.items()}
-    order = list(units)  # pool order of this rank
-    # 1.
-    mine = torch.zeros(1 + pool_bricks, 4, dtype=torch.int32)
-    mine[0, 0] = len(order)
-    if order:
-        mine[1:1 + len(order), :3] = torch.tensor(order, dtype=torch.int32)
-    gathered = [torch.zeros_like(mine) for _ in range(world)]
-    dist.all_gather(gathered, mine, group=group)
-    # 2.
-    if receives:
-        for r in range(world):
-            if r == rank:
-                continue
-            for k in gathered[r][1:1 + int(gathered[r][0, 0])].tolist():
-                key = tuple(k[:3])
-                if key not in units:
-                    units[key] = np.zeros((BRICK_VOXELS, 2), np.float32)
-                    order.append(key)
-    # 3.
-    canon = torch.zeros(1 + pool_bricks, 4, dtype=torch.int32)
-    if rank == canon_rank:
-        canon[0, 0] = len(order)
-        canon[1:1 + len(order), :3] = torch.tensor(order, dtype=torch.int32)
-    dist.broadcast(canon, src=canon_rank if group is None else dist.get_global_rank(group, canon_rank), group=group)
-    n = int(canon[0, 0])
-    canon_keys = [tuple(k[:3]) for k in canon[1:1 + n].tolist()]
-    # 4.
-    packed = torch.zeros(n, BRICK_VOXELS, 2, dtype=torch.float32)
-    for i, key in enumerate(canon_keys):
-        if key in units:
-            tw = units[key]
-            packed[i, :, 0] = torch.from_numpy(tw[:, 0] * tw[:, 1])
-            packed[i, :, 1] = torch.from_numpy(tw[:, 1])
-    # 5.
-    if dst is None:
-        dist.all_reduce(packed, op=dist.ReduceOp.SUM, group=group)
-    else:
-        dist.reduce(packed, dst=canon_rank if group is None else dist.get_global_rank(group, canon_rank), op=dist.ReduceOp.SUM,
-                    group=group)
-    # 6.
-    if receives:
-        p = packed.numpy()
-        for i, key in enumerate(canon_keys):
-            w = p[i, :, 1]
-            units[key] = np.stack([np.where(w > 0, p[i, :, 0] / np.maximum(w, 1e-30), 0).astype(np.float32), w], -1)
-    return units
-
-
-def merge_bricks_reference(volumes_tw):
-    """Host-side statement of the cross-rank merge (used by the CPU gloo tests):
-    given per-rank [n,4096,2] (mean, weight) arrays returns the merged (mean, weight)."""
-    total_w = sum(tw[..., 1] for tw in volumes_tw)
-    total_s = sum(tw[..., 0] * tw[..., 1] for tw in volumes_tw)
-    mean = np.where(total_w > 0, total_s / np.maximum(total_w, 1e-30), 0.0).astype(np.float32)
-    return np.stack([mean, total_w.astype(np.float32)], axis=-1)
 
 
 def shard_views(num_views: int, rank: int, world_size: int):

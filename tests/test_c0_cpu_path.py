@@ -84,25 +84,37 @@ def test_fused_volume_and_mesh_recover_the_surface(c0, oracle):
     assert 0.55 < np.percentile(r, 1) and np.percentile(r, 99) < 1.05 and abs(np.median(r) - 0.8) < 0.03, np.percentile(r, [1, 50, 99])
 
 
-def test_view_sharding_and_merge_equal_sequential_fusion(c0, oracle):
-    """SURVEY 8(e) on the C0 case: ranks take views round-robin, volumes are merged as (sum tsdf*w, sum w)."""
-    from gs2mesh_b200.tsdf import merge_bricks_reference, shard_views
+def test_shard_views_round_robin():
+    from gs2mesh_b200.tsdf import shard_views
+
+    assert shard_views(7, 0, 2) == [0, 2, 4, 6] and shard_views(7, 1, 2) == [1, 3, 5]
+    got = sorted(v for r in range(8) for v in shard_views(500, r, 8))
+    assert got == list(range(500))
+    assert max(len(shard_views(500, r, 8)) for r in range(8)) - min(len(shard_views(500, r, 8)) for r in range(8)) <= 1
+    assert shard_views(3, 5, 8) == []
+
+
+def test_view_shards_merged_by_merge_oracle_equal_sequential_fusion(c0, oracle):
+    """SURVEY 8(e) on the C0 case: ranks take views round-robin, and the multi-GPU merge's host restatement
+    (tests/merge_oracle.py) of the two ranks' volumes opens the sequential fusion's units with the same weights and tsdf."""
+    from gs2mesh_b200.tsdf import shard_views
+    from tests.merge_oracle import merge_oracle
 
     cfg = c0["cfg"]
     vl = 2.0 / cfg["tsdf_res"]
     trunc = max(0.04, 3 * vl)
-    nb = cfg["tsdf_res"] // 16
-    origin, count = (-(nb // 2),) * 3, (nb,) * 3
-    seq = oracle.OracleTSDFVolume(vl, trunc, with_color=False)
-    for i in range(cfg["pairs"]):
-        _integrate(c0, seq, i)
-    parts = []
-    for rank in range(2):
+
+    def fuse(views):
+        """{(bx,by,bz): (tsdf, weight) [4096,2]} of every unit the views open."""
         vol = oracle.OracleTSDFVolume(vl, trunc, with_color=False)
-        for i in shard_views(cfg["pairs"], rank, 2):
+        for i in views:
             _integrate(c0, vol, i)
-        parts.append(vol.export_bricks(origin, count)[0])
-    merged = merge_bricks_reference(parts)
-    ref = seq.export_bricks(origin, count)[0]
-    np.testing.assert_array_equal(merged[..., 1], ref[..., 1])
-    assert np.abs(merged[..., 0] - ref[..., 0]).max() < 1e-6
+        return {tuple(int(v) for v in k): np.stack(vol.unit_data(i)[:2], -1) for i, k in enumerate(vol.unit_indices())}
+
+    ref = fuse(range(cfg["pairs"]))
+    ranks = [{k: (tw, None) for k, tw in fuse(shard_views(cfg["pairs"], rank, 2)).items()} for rank in range(2)]
+    merged = merge_oracle(ranks, None, len(set(ranks[0]) | set(ranks[1])))[0].merged
+    assert set(merged) == set(ref)
+    for k, (tw, _) in merged.items():  # two ranks: one candidate per voxel
+        np.testing.assert_array_equal(tw[0][:, 1], ref[k][:, 1])
+        assert np.abs(tw[0][:, 0] - ref[k][:, 0]).max() < 1e-6

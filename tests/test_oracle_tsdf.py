@@ -99,31 +99,35 @@ def _rot_y(deg):
     return e
 
 
-def test_view_order_independence_and_sharded_merge(oracle):
-    from gs2mesh_b200.tsdf import merge_bricks_reference
+def test_view_order_independence_and_merge_oracle_of_shards(oracle):
+    """Fusing the views in another order, or in two shards merged by the multi-GPU merge's host restatement, opens the same
+    units as sequential fusion, with bit-equal weights and tsdf within 1e-6."""
+    from tests.merge_oracle import merge_oracle
 
     views = []
     for k, ang in enumerate([-8, -3, 4, 9]):
         e = _rot_y(ang)
         e[2, 3] = 0.1 * k
         views.append((_plane(1.0 + 0.01 * k), e))
-    b0, nb = (-4, -4, -2), (8, 8, 8)
 
     def fuse(order):
+        """{(bx,by,bz): (tsdf, weight) [4096,2]} of every unit the views open."""
         vol = oracle.OracleTSDFVolume(VL, TRUNC, with_color=False)
         for i in order:
             vol.integrate(views[i][0], None, W, H, FX, FY, CX, CY, views[i][1])
-        tw, alloc, outside = vol.export_bricks(b0, nb)
-        assert outside == 0
-        return tw
+        return {tuple(int(v) for v in k): np.stack(vol.unit_data(i)[:2], -1) for i, k in enumerate(vol.unit_indices())}
+
+    def same(got, want):
+        assert set(got) == set(want)
+        for k in want:
+            np.testing.assert_array_equal(got[k][:, 1], want[k][:, 1])
+            np.testing.assert_allclose(got[k][:, 0], want[k][:, 0], atol=1e-6)
 
     seq = fuse([0, 1, 2, 3])
-    perm = fuse([2, 0, 3, 1])
-    np.testing.assert_array_equal(seq[..., 1], perm[..., 1])
-    np.testing.assert_allclose(seq[..., 0], perm[..., 0], atol=1e-6)
-    merged = merge_bricks_reference([fuse([0, 2]), fuse([1, 3])])
-    np.testing.assert_array_equal(merged[..., 1], seq[..., 1])
-    np.testing.assert_allclose(merged[..., 0], seq[..., 0], atol=1e-6)
+    same(fuse([2, 0, 3, 1]), seq)
+    shards = [{k: (tw, None) for k, tw in fuse(order).items()} for order in ([0, 2], [1, 3])]
+    merged = merge_oracle(shards, None, len(set(shards[0]) | set(shards[1])))[0].merged
+    same({k: tw[0] for k, (tw, _) in merged.items()}, seq)  # two ranks: one candidate per voxel
 
 
 def _blob_mask(rng, h, w):
