@@ -3,7 +3,7 @@
 PyTorch is used for device memory and streams only; all compute happens in
 libgs2mesh_b200.so.  Mirrors the marshalling the reference does in
 DGR/rasterize_points.cu:35-115 (allocate outputs, hand raw pointers to the kernels),
-with one persistent grow-only scratch block per device instead of three byte tensors that
+with a grow-only `Scratch` block per frame in flight instead of three byte tensors that
 are resized on every call (rasterize_points.cu:27-33, 71-75).
 """
 from __future__ import annotations
@@ -21,47 +21,69 @@ from ._lib import GsbRasterArgs, ptr
 # (transmittance bit-identical to the reference binary; ~8 % slower per frame).
 DEFAULT_FLAGS = _lib.RASTER_EXACT_TILE_CULL | _lib.RASTER_FAST_EXP
 EXACT_EXP_FLAGS = _lib.RASTER_EXACT_TILE_CULL
-# first guess of the binning capacity of a scratch block: instances per Gaussian / floor (tests shrink these to provoke overflow)
+# first guess of the binning capacity of a block that has not seen a frame: instances per Gaussian / floor
 GUESS_PER_GAUSSIAN = 4
 MIN_GUESS = 1 << 20
 
 
-class _Scratch:
-    """Grow-only workspace + binning capacity, and the instance counts of calls that do not ask for them."""
+def capacity_for(need: int) -> int:
+    """Binning capacity for frames that need up to `need` instances (what `num_rendered[0]` reports, also for a frame
+    that overflowed)."""
+    return int(need * 1.1) + 4096
 
-    def __init__(self, device):
+
+class Scratch:
+    """Scratch block of one frame in flight: the binning workspace, its capacity for one (P, W, H), and the int64[4]
+    counts buffer of synchronous calls that do not ask for counts.
+
+    Two frames in flight at the same time need two blocks; the owner of the streams a block is used on orders its reuse.
+    Its tensors are recorded on every stream they are enqueued on, so releasing them -- on growth, on a new frame shape or
+    when the owner drops the block -- waits for the work those streams hold at that moment."""
+
+    def __init__(self, device, max_instances=0):
         self.device = device
-        self.buf: Optional[torch.Tensor] = None
-        self.max_instances = 0
+        self.max_instances = int(max_instances)  # 0: the first frame starts from the first guess
         self.key = None
-        self.counts = torch.zeros(4, dtype=torch.int64, device=device)
+        self.workspace: Optional[torch.Tensor] = None
+        self.counts: Optional[torch.Tensor] = None
+        self._recorded = set()  # handles of the streams the current tensors are recorded on
 
-    def ensure(self, P, W, H, min_instances):
-        """Workspace for a P-Gaussian W x H frame with room for at least `min_instances` instances; the capacity of a
-        frame shape never shrinks."""
+    def ensure(self, P, W, H, min_instances, streams):
+        """Workspace for a P-Gaussian W x H frame with room for at least `min_instances` instances, enqueued on `streams`
+        (its work starts on streams[0]); the capacity for one frame shape never shrinks."""
         key = (P, W, H)
-        max_instances = max(self.max_instances if key == self.key else 0, GUESS_PER_GAUSSIAN * P, MIN_GUESS, int(min_instances))
-        if self.buf is None or key != self.key or max_instances > self.max_instances:
+        if self.key not in (None, key):
+            self.max_instances = 0
+        max_instances = max(self.max_instances or max(GUESS_PER_GAUSSIAN * P, MIN_GUESS), int(min_instances))
+        if self.workspace is None or key != self.key or max_instances > self.max_instances:
             need = _lib.lib().gsb_raster_workspace_bytes(P, W, H, max_instances)
-            if self.buf is None or self.buf.numel() < need:
-                self.buf = None  # release before re-allocating
-                self.buf = torch.empty(need, dtype=torch.uint8, device=self.device)
+            if self.workspace is None or self.workspace.numel() < need:
+                self.workspace = None  # release before re-allocating
+                # on the stream the frame starts on: the memory may still be in use by work queued there, and the
+                # frame's work on its other streams is ordered behind its start
+                with torch.cuda.stream(streams[0]):
+                    self.workspace = torch.empty(need, dtype=torch.uint8, device=self.device)
+                    if self.counts is None:
+                        self.counts = torch.zeros(4, dtype=torch.int64, device=self.device)
+                self._recorded = set()
             self.max_instances = max_instances
             self.key = key
-        return self.buf
+        for s in streams:
+            if s.cuda_stream not in self._recorded:
+                self._recorded.add(s.cuda_stream)
+                self.workspace.record_stream(s)
+                self.counts.record_stream(s)
+        return self.workspace
 
 
-_scratch = {}
+_scratch = {}  # (device index, stream handle) -> the block of synchronous single-view calls that bring none
 
 
-def _scratch_for(device, stream=None, eye=0) -> _Scratch:
-    """One scratch block per (device, stream, eye): frames enqueued on different streams may overlap, and the two eyes of a
-    stereo pair are in flight together even when they share a stream."""
-    dev = torch.device(device)
-    idx = dev.index if dev.index is not None else torch.cuda.current_device()
-    key = (idx, (stream if stream is not None else torch.cuda.current_stream(idx)).cuda_stream, eye)
+def _default_scratch(device, stream) -> Scratch:
+    """The block of synchronous single-view calls that bring none, one per (device, stream): the stream orders its reuse."""
+    key = (device.index, stream.cuda_stream)
     if key not in _scratch:
-        _scratch[key] = _Scratch(torch.device("cuda", idx))
+        _scratch[key] = Scratch(device)
     return _scratch[key]
 
 
@@ -85,8 +107,8 @@ def rasterize_forward(*, means3D, opacities, viewmatrix, projmatrix, campos, bg,
                       shs=None, colors_precomp=None, scales=None, rotations=None, cov3D_precomp=None, sh_degree=0,
                       scale_modifier=1.0, prefiltered=False, flags=DEFAULT_FLAGS, want_depth=True, want_final_T=True,
                       want_radii=True, want_counts=False, out_color=None, out_depth=None, out_final_T=None,
-                      async_mode=False, counts_out=None, min_instances=0):
-    """One forward rasterization on the current CUDA stream.
+                      async_mode=False, counts_out=None, min_instances=0, scratch: Optional[Scratch] = None):
+    """One forward rasterization on the current CUDA stream, in the scratch block `scratch`.
 
     Returns dict(color[3,H,W], depth[H,W]|None, final_T[H,W]|None, radii[P]|None,
     counts (int64[4]: binned instances, reference-equivalent instances, overflow flag, large tiles)|None).
@@ -95,7 +117,13 @@ def rasterize_forward(*, means3D, opacities, viewmatrix, projmatrix, campos, bg,
     undersized scratch block can be grown and the frame redone transparently.
     async_mode=True: nothing waits; pass `counts_out` (int64[4], device or pinned host memory) and check
     counts_out[2] == 0 after your own synchronisation (see Renderer.check_status()).
+    An asynchronous call (async_mode, or RASTER_ASYNC in `flags`) needs a `scratch` block of its own; a synchronous call
+    without one uses the block of the current stream.
     """
+    flags = int(flags) | (_lib.RASTER_ASYNC if async_mode else 0)
+    asynchronous = bool(flags & _lib.RASTER_ASYNC)
+    if asynchronous and scratch is None:
+        raise ValueError("an asynchronous rasterize_forward needs its own scratch block (scratch=Scratch(device))")
     if means3D.ndim != 2 or means3D.shape[1] != 3:
         raise RuntimeError("means3D must have dimensions (num_points, 3)")  # rasterize_points.cu:57-59
     device = means3D.device
@@ -129,25 +157,25 @@ def rasterize_forward(*, means3D, opacities, viewmatrix, projmatrix, campos, bg,
         final_T = (out_final_T if out_final_T is not None else torch.empty(H, W, **f32)) if want_final_T else None
         radii = torch.empty(P, dtype=torch.int32, device=device) if want_radii else None
         counts = counts_out if counts_out is not None else (torch.zeros(4, dtype=torch.int64, device=device) if want_counts else None)
-        scratch = _scratch_for(device)
-        status = counts if counts is not None else scratch.counts  # [0] is the frame's instance need, also on overflow
-        stream = C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
+        st = torch.cuda.current_stream(device)
+        if scratch is None:
+            scratch = _default_scratch(device, st)
+        stream = C.c_void_p(st.cuda_stream)
         L = _lib.lib()
-        if async_mode:
-            flags = int(flags) | _lib.RASTER_ASYNC
-        for attempt in range(1 if async_mode else 3):
-            ws = scratch.ensure(P, W, H, min_instances)
+        for attempt in range(1 if asynchronous else 3):
+            ws = scratch.ensure(P, W, H, min_instances, (st,))
+            status = counts if counts is not None else scratch.counts  # [0] is the frame's instance need, also on overflow
             args = GsbRasterArgs(
                 P=P, sh_degree=int(sh_degree), sh_coeffs=M, width=W, height=H, background=ptr(bg), means3D=ptr(means3D),
                 shs=ptr(shs), colors_precomp=ptr(colors_precomp), opacities=ptr(opacities), scales=ptr(scales),
                 rotations=ptr(rotations), cov3D_precomp=ptr(cov3D_precomp), scale_modifier=float(scale_modifier),
                 viewmatrix=ptr(viewmatrix), projmatrix=ptr(projmatrix), cam_pos=ptr(campos), tan_fovx=float(tan_fovx),
-                tan_fovy=float(tan_fovy), prefiltered=int(bool(prefiltered)), flags=int(flags), out_color=ptr(color),
+                tan_fovy=float(tan_fovy), prefiltered=int(bool(prefiltered)), flags=flags, out_color=ptr(color),
                 out_depth=ptr(depth), out_final_T=ptr(final_T), radii=ptr(radii), num_rendered=ptr(status),
                 workspace=ptr(ws), workspace_bytes=ws.numel(), max_instances=scratch.max_instances)
             rc = L.gsb_raster_forward(C.byref(args), stream)
-            if rc == _lib.GSB_ERR_WORKSPACE and attempt < 2 and not async_mode:
-                min_instances = int(int(status[0]) * 1.25) + 1024
+            if rc == _lib.GSB_ERR_WORKSPACE and attempt < 2 and not asynchronous:
+                min_instances = capacity_for(int(status[0]))
                 continue
             _lib.check(rc)
             break
@@ -155,15 +183,20 @@ def rasterize_forward(*, means3D, opacities, viewmatrix, projmatrix, campos, bg,
 
 
 def rasterize_forward_pair(*, means3D, opacities, shs, scales, rotations, sh_degree, bg, width, height, eyes, streams,
-                           flags=DEFAULT_FLAGS, shared_depth=False, scale_modifier=1.0, min_instances=0):
+                           scratch=None, flags=DEFAULT_FLAGS, shared_depth=False, scale_modifier=1.0, min_instances=0):
     """Both eyes of a stereo pair through `gsb_raster_forward_pair` (one fused preprocess pass over the Gaussian
     parameters; with `shared_depth` also one depth sort).  Always asynchronous.
 
     eyes: two dicts with viewmatrix[16], projmatrix[16], campos[3] (device), tan_fovx, tan_fovy, out_color[3,H,W],
           out_depth / out_final_T ([H,W] or None), counts_out (int64[4], device or pinned host, or None).
-    streams: (left, right) torch streams; the shared part runs on the left one, each eye has its own scratch block.
+    streams: (left, right) torch streams; the shared part runs on the left one.
+    scratch: (left, right) `Scratch` blocks, one per eye.  The shared part writes both on the left stream, and each
+    eye's binning and blend read them on its own stream, so both blocks are recorded on both streams.  The left stream
+    first waits for the right one: a pair may reuse the blocks of the previous pair on the same streams.
     The caller checks counts_out[2] (scratch overflow) and counts_out[3] (shared_depth claimed but depths differ) after
     its own synchronisation."""
+    if scratch is None:
+        raise ValueError("rasterize_forward_pair needs one scratch block per eye (scratch=(left, right))")
     device = means3D.device
     P = means3D.shape[0]
     W, H = int(width), int(height)
@@ -177,10 +210,11 @@ def rasterize_forward_pair(*, means3D, opacities, shs, scales, rotations, sh_deg
                         eye[k].zero_()
         return
     with torch.cuda.device(device):
+        if streams[1] != streams[0]:
+            streams[0].wait_stream(streams[1])
         blocks = []
-        for s_, (eye, st) in enumerate(zip(eyes, streams)):
-            scratch = _scratch_for(device, st, s_)
-            ws = scratch.ensure(P, W, H, min_instances)
+        for eye, block in zip(eyes, scratch):
+            ws = block.ensure(P, W, H, min_instances, streams)
             fl = int(flags) | _lib.RASTER_ASYNC | (_lib.RASTER_PAIR_SHARED_DEPTH if shared_depth else 0)
             blocks.append(GsbRasterArgs(
                 P=P, sh_degree=int(sh_degree), sh_coeffs=M, width=W, height=H, background=ptr(bg), means3D=ptr(means3D),
@@ -190,7 +224,7 @@ def rasterize_forward_pair(*, means3D, opacities, shs, scales, rotations, sh_deg
                 tan_fovy=float(eye["tan_fovy"]), prefiltered=0, flags=fl, out_color=ptr(eye["out_color"]),
                 out_depth=ptr(eye.get("out_depth")), out_final_T=ptr(eye.get("out_final_T")), radii=None,
                 num_rendered=ptr(eye.get("counts_out")), workspace=ptr(ws), workspace_bytes=ws.numel(),
-                max_instances=scratch.max_instances))
+                max_instances=block.max_instances))
         _lib.check(L.gsb_raster_forward_pair(C.byref(blocks[0]), C.byref(blocks[1]), C.c_void_p(streams[0].cuda_stream),
                                              C.c_void_p(streams[1].cuda_stream)))
 

@@ -47,6 +47,15 @@ DEFAULT_COPY_STREAMS = 0
 DEFAULT_SPARE_BUFFER_SETS = 0
 
 
+class _StreamSet(list):
+    """The (left, right) streams a stereo pair is rendered on, and the scratch blocks of its two eyes (`scratch`): the
+    blocks are only ever used by the pair in flight on these streams."""
+
+    def __init__(self, streams, scratch):
+        super().__init__(streams)
+        self.scratch = scratch
+
+
 class _PairReady:
     """Completion handle of an asynchronously rendered pair (render_image_pair(..., wait=False)).  synchronize() waits for
     both eyes and -- like the synchronous call -- transparently re-renders the pair if its binning scratch turned out too
@@ -168,10 +177,14 @@ class Renderer:
         # per-(view, side) rasterizer status words, written by the GPU straight into pinned host memory
         self._status = torch.zeros(len(self.cameras), 2, 4, dtype=torch.int64).pin_memory()
         self._min_instances = 0
+        # the block of the synchronous single-view calls; the serial pair path (both eyes on the caller's stream) uses it
+        # for its left eye, since both only ever run on the caller's stream
+        self._view_block = rast.Scratch(dev)
+        self._serial_blocks = (self._view_block, rast.Scratch(dev))
         self._ready = True
         self.calibrate_capacity()
 
-    def calibrate_capacity(self, sample_views=None, slack=1.1):
+    def calibrate_capacity(self, sample_views=None):
         """Size the binning scratch once so that the hot loop can run without ever waiting for the GPU (the reference
         re-sizes -- and blocks -- inside every frame, rasterizer_impl.cu:281-285).  By default EVERY view of the rig is
         rendered once (instance counts are deterministic per camera), so a frame of this camera set cannot outgrow the
@@ -184,7 +197,7 @@ class Renderer:
             views = sorted(set(int(round(k * (n - 1) / max(sample_views - 1, 1))) for k in range(sample_views)))
         counts = [self.render_view(i, s, want_counts=True)["counts"] for i in views for s in range(2)]  # grow-and-redo renders
         worst = int(torch.stack(counts)[:, 0].max().item()) if counts else 0
-        self._min_instances = int(worst * slack) + 4096
+        self._min_instances = rast.capacity_for(worst)
 
     def check_status(self, views=None):
         """After a synchronisation: raise if any asynchronously rendered frame is invalid (binning scratch too small, or a
@@ -194,7 +207,7 @@ class Renderer:
         bad = ((st[..., 2] != 0) | (st[..., 3] != 0)).nonzero()
         if len(bad):
             need = int(st[..., 0].max().item())
-            self._min_instances = max(self._min_instances, int(need * 1.25))
+            self._min_instances = max(self._min_instances, rast.capacity_for(need))
             raise RuntimeError(f"{len(bad)} frame(s) are invalid (needed up to {need} instances of binning scratch); "
                                "capacity has been raised, render them again")
 
@@ -203,7 +216,7 @@ class Renderer:
         st = self._status[camera_number]
         ok = True
         if bool((st[:, 2] != 0).any()):
-            self._min_instances = max(self._min_instances, int(int(st[:, 0].max().item()) * 1.25) + 4096)
+            self._min_instances = max(self._min_instances, rast.capacity_for(int(st[:, 0].max().item())))
             ok = False
         if bool((st[:, 3] != 0).any()):
             self._shared_depth[camera_number] = False
@@ -225,8 +238,9 @@ class Renderer:
         return self._bufs[key]
 
     def render_view(self, camera_number, side, *, want_depth=False, out_color=None, out_depth=None, out_final_T=None,
-                    flags=None, want_counts=False, async_mode=False):
-        """One forward rasterization of view `camera_number`, side 0 (left) / 1 (right)."""
+                    flags=None, want_counts=False, async_mode=False, scratch=None):
+        """One forward rasterization of view `camera_number`, side 0 (left) / 1 (right), on the current stream.  A
+        synchronous call without `scratch` uses the renderer's single-view block; an asynchronous one needs its own."""
         if not self._ready:
             raise RuntimeError("call prepare_renderer() first")
         if flags is None:
@@ -239,10 +253,11 @@ class Renderer:
             scales=self.scales, rotations=self.rotations, sh_degree=self.sh_degree, scale_modifier=1.0, flags=flags,
             want_depth=want_depth, want_final_T=want_depth, want_radii=False, want_counts=want_counts,
             out_color=out_color, out_depth=out_depth, out_final_T=out_final_T, async_mode=async_mode,
-            counts_out=self._status[camera_number, side] if async_mode else None, min_instances=self._min_instances)
+            counts_out=self._status[camera_number, side] if async_mode else None, min_instances=self._min_instances,
+            scratch=scratch if scratch is not None or async_mode else self._view_block)
 
     def _enqueue_pair(self, camera_number, b, streams):
-        """Both eyes of one view into buffer set `b`: rasterize (+ u8 conversion) on `streams` (left, right)."""
+        """Both eyes of one view into buffer set `b`: rasterize (+ u8 conversion) on the _StreamSet `streams`."""
         mode = os.environ.get("GSB_PAIR_MODE", "fused")  # A/B switch: fused | noshare (fused preprocess, two depth sorts) | separate
         flags = rast.DEFAULT_FLAGS if self.fast_exp else rast.EXACT_EXP_FLAGS
         self._status[camera_number].zero_()
@@ -251,7 +266,7 @@ class Renderer:
                 with torch.cuda.stream(streams[s]):
                     self.render_view(camera_number, s, want_depth=(s == 0), out_color=b["color"][s],
                                      out_depth=b["depth"] if s == 0 else None, out_final_T=b["final_T"] if s == 0 else None,
-                                     async_mode=True)
+                                     async_mode=True, scratch=streams.scratch[s])
         else:
             eyes = []
             for s in range(2):
@@ -263,7 +278,7 @@ class Renderer:
             vt = self._views[camera_number][0]
             rast.rasterize_forward_pair(means3D=self.means3D, opacities=self.opacity, shs=self.shs, scales=self.scales,
                                         rotations=self.rotations, sh_degree=self.sh_degree, bg=self.background, width=vt.width,
-                                        height=vt.height, eyes=eyes, streams=streams, flags=flags,
+                                        height=vt.height, eyes=eyes, streams=streams, scratch=streams.scratch, flags=flags,
                                         shared_depth=self._shared_depth[camera_number] and mode != "noshare",
                                         min_instances=self._min_instances)
         for s in range(2):
@@ -303,11 +318,12 @@ class Renderer:
                 spare = int(self.spare_buffer_sets)
                 nslots = depth + 2 + spare
                 slot = self._call_index % nslots
-                if not hasattr(self, "_side_streams") or len(self._side_streams) != depth:
+                if not hasattr(self, "_stream_sets") or len(self._stream_sets) != depth:
                     # `pairs_in_flight` sets of (left, right) streams, used round-robin: consecutive pairs run on
-                    # different stream sets (each stream has its own scratch), so pair n+1's latency-bound binning
+                    # different stream sets (each with its own scratch blocks), so pair n+1's latency-bound binning
                     # kernels fill the gaps of pair n's blend kernels
-                    self._side_streams = [[torch.cuda.Stream(dev), torch.cuda.Stream(dev)] for _ in range(depth)]
+                    self._stream_sets = [_StreamSet([torch.cuda.Stream(dev), torch.cuda.Stream(dev)],
+                                                    (rast.Scratch(dev), rast.Scratch(dev))) for _ in range(depth)]
                 if not hasattr(self, "_entry_events") or len(self._entry_events) != nslots:
                     main.synchronize()  # (re)configuration only: nothing may still use the old rotation
                     self._call_index = 0
@@ -321,7 +337,7 @@ class Renderer:
                 # c - nslots + depth + 1 = c - 1 - spare was entered) was enqueued on the caller's stream before that entry
                 gate = self._entry_events[(self._call_index - 1 - spare) % nslots] if self._call_index > spare else None
                 self._entry_events[slot] = entry
-                streams = self._side_streams[self._call_index % depth]
+                streams = self._stream_sets[self._call_index % depth]
                 if self.copy_streams and to_host:
                     if not hasattr(self, "_copy_streams") or len(self._copy_streams) != depth:
                         self._copy_streams = [[torch.cuda.Stream(dev), torch.cuda.Stream(dev)] for _ in range(depth)]
@@ -335,7 +351,7 @@ class Renderer:
                         st.wait_event(done)
             else:
                 b = self._buffers(vt.width, vt.height)
-                streams = [main, main]
+                streams = _StreamSet([main, main], self._serial_blocks)
 
             # the streams whose completion means "this pair is done": the copy streams when the frames travel on their own
             # streams (each copy is ordered behind everything its eye's render stream holds at that point), else the render streams

@@ -96,7 +96,7 @@ def test_wrong_shared_depth_claim_is_flagged_and_repaired(gsb_lib, cuda_device, 
         r.check_status([view])
 
 
-def test_scratch_overflow_is_repaired_transparently(gsb_lib, cuda_device, rig, monkeypatch):
+def test_undersized_renderer_scratch_is_repaired_transparently(gsb_lib, cuda_device, rig):
     """The reference resizes its binning buffer inside every frame (rasterizer_impl.cu:281-285); here an undersized scratch is
     detected from the frame's status word and the pair is rendered again -- on the synchronous path and on the handle of the
     asynchronous one -- instead of raising."""
@@ -106,14 +106,13 @@ def test_scratch_overflow_is_repaired_transparently(gsb_lib, cuda_device, rig, m
     good = [_grab(r.render_image_pair(i, to_host=True)) for i in (0, 1)]
     need = int(r._status[0, :, 0].max())
     assert need > 20000
-    monkeypatch.setattr(rast, "MIN_GUESS", 1024)
-    monkeypatch.setattr(rast, "GUESS_PER_GAUSSIAN", 0)
 
     def shrink():
         import torch
 
         torch.cuda.synchronize()
-        rast._scratch.clear()  # forget the grown scratch blocks
+        for st in r._stream_sets:  # replace the grown scratch blocks with 1024-instance ones
+            st.scratch = (rast.Scratch(cuda_device, max_instances=1024), rast.Scratch(cuda_device, max_instances=1024))
         r._min_instances = 1
 
     # synchronous call: rendered, found too small, scratch grown, rendered again -- all inside the call
@@ -190,7 +189,7 @@ def test_in_memory_handoff_equals_file_round_trip(oracle, gsb_lib, cuda_device, 
 
 
 @pytest.mark.parametrize("num_points,W,H,deg", [(4099, 333, 250, 3), (777, 250, 130, 1), (33, 64, 48, 0)])
-def test_pair_entry_point_on_ragged_inputs(gsb_lib, cuda_device, num_points, W, H, deg):
+def test_pair_entry_point_on_ragged_inputs_in_caller_blocks(gsb_lib, cuda_device, num_points, W, H, deg):
     """`gsb_raster_forward_pair` through the ctypes stub against two `gsb_raster_forward` calls on awkward shapes: a Gaussian
     count that is no multiple of the warp size (the last warp takes the plain-load path), ragged tile rows / columns, lower SH
     degrees; with and without a shared depth order; eyes on one stream and on two."""
@@ -219,6 +218,7 @@ def test_pair_entry_point_on_ragged_inputs(gsb_lib, cuda_device, num_points, W, 
             want.append({k: o[k].clone() for k in ("color", "depth", "final_T", "counts")})
         main = torch.cuda.current_stream(dev)
         side = torch.cuda.Stream(dev)
+        scratch = (rast.Scratch(dev), rast.Scratch(dev))
         for streams in ((main, main), (main, side)):
             for claim in ((True, False) if shared else (False,)):
                 eyes = []
@@ -228,7 +228,7 @@ def test_pair_entry_point_on_ragged_inputs(gsb_lib, cuda_device, num_points, W, 
                                      out_final_T=torch.empty(H, W, device=dev), counts_out=torch.zeros(4, dtype=torch.int64, device=dev)))
                 side.wait_stream(main)
                 rast.rasterize_forward_pair(means3D=means, opacities=op, shs=shs, scales=sc, rotations=ro, sh_degree=deg, bg=bg,
-                                            width=W, height=H, eyes=eyes, streams=streams, shared_depth=claim)
+                                            width=W, height=H, eyes=eyes, streams=streams, scratch=scratch, shared_depth=claim)
                 torch.cuda.synchronize()
                 for e, w in zip(eyes, want):
                     assert int(e["counts_out"][2]) == 0 and int(e["counts_out"][3]) == 0
@@ -241,6 +241,44 @@ def test_pair_entry_point_on_ragged_inputs(gsb_lib, cuda_device, num_points, W, 
                  tan_fovy=vts[0].tan_fovy)
     eyes = [dict(empty, out_color=torch.ones(3, H, W, device=dev), out_depth=None, out_final_T=None, counts_out=None) for _ in range(2)]
     rast.rasterize_forward_pair(means3D=means[:0], opacities=op[:0], shs=shs[:0], scales=sc[:0], rotations=ro[:0], sh_degree=deg, bg=bg,
-                                width=W, height=H, eyes=eyes, streams=(main, main))
+                                width=W, height=H, eyes=eyes, streams=(main, main), scratch=scratch)
     torch.cuda.synchronize()
     assert all(float(e["out_color"].abs().max()) == 0.0 for e in eyes)
+
+
+def test_pair_scratch_is_released_with_its_blocks(gsb_lib, cuda_device, rig):
+    """The wrapper keeps nothing for the streams it ran on: once the caller drops the blocks of a pair rendered on fresh
+    streams, the device memory they took is free again."""
+    import gc
+
+    import torch
+
+    from gs2mesh_b200 import camera as cam
+    from gs2mesh_b200 import rasterizer as rast
+
+    cloud, rigs, _ = rig
+    dev = cuda_device
+    t = lambda a: torch.as_tensor(np.ascontiguousarray(a, dtype=np.float32)).to(dev)
+    means, op, shs, sc, ro = t(cloud.xyz), t(cloud.opacity).reshape(-1), t(cloud.features), t(cloud.scaling), t(cloud.rotation)
+    eyes = []
+    for side in ("left", "right"):
+        vt = cam.view_transforms_from_camera(rigs[0][side])
+        rec = t(vt.packed())
+        eyes.append(dict(viewmatrix=rec[0:16], projmatrix=rec[16:32], campos=rec[32:35], tan_fovx=vt.tan_fovx,
+                         tan_fovy=vt.tan_fovy, out_color=torch.empty(3, H, W, device=dev),
+                         counts_out=torch.zeros(4, dtype=torch.int64, device=dev)))
+    bg = torch.zeros(3, device=dev)
+    streams = (torch.cuda.Stream(dev), torch.cuda.Stream(dev))
+    for st in streams:
+        st.wait_stream(torch.cuda.current_stream(dev))
+    torch.cuda.synchronize()
+    before = torch.cuda.memory_allocated(dev)
+    scratch = (rast.Scratch(dev), rast.Scratch(dev))
+    rast.rasterize_forward_pair(means3D=means, opacities=op, shs=shs, scales=sc, rotations=ro, sh_degree=cloud.sh_degree, bg=bg,
+                                width=W, height=H, eyes=eyes, streams=streams, scratch=scratch)
+    assert torch.cuda.memory_allocated(dev) > before
+    del scratch
+    gc.collect()
+    torch.cuda.synchronize()
+    assert torch.cuda.memory_allocated(dev) == before
+    assert all(int(e["counts_out"][2]) == 0 for e in eyes) and float(eyes[0]["out_color"].abs().max()) > 0

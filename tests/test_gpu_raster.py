@@ -196,7 +196,7 @@ def test_binned_sort_equals_reference_shaped_sort(gsb_lib, cuda_device):
             assert new["counts"][2] == 0
 
 
-def test_async_mode_reports_overflow_in_status_word(gsb_lib, cuda_device):
+def test_async_mode_in_caller_block_reports_counts_in_status_word(gsb_lib, cuda_device):
     import torch
 
     from gs2mesh_b200 import rasterizer as rast
@@ -210,7 +210,7 @@ def test_async_mode_reports_overflow_in_status_word(gsb_lib, cuda_device):
               tan_fovy=vt.tan_fovy, shs=t(g.features), scales=t(g.scaling), rotations=t(g.rotation), sh_degree=3)
     sync = rast.rasterize_forward(**kw, want_counts=True)
     torch.cuda.synchronize()
-    out = rast.rasterize_forward(**kw, async_mode=True, counts_out=status)
+    out = rast.rasterize_forward(**kw, async_mode=True, counts_out=status, scratch=rast.Scratch(dev))
     torch.cuda.synchronize()
     assert status[2] == 0 and status[0] == sync["counts"][0].item() and status[1] == sync["counts"][1].item()
     assert torch.equal(out["color"], sync["color"])
@@ -355,7 +355,7 @@ def test_workspace_too_small_reports_need_in_num_rendered(gsb_lib, cuda_device):
         assert rc == _lib.GSB_OK and torch.isfinite(col).all() and float(col.mean()) > 0.01
 
 
-def test_wrapper_grows_undersized_scratch_and_renders_again(gsb_lib, cuda_device, monkeypatch):
+def test_wrapper_grows_undersized_scratch_and_renders_again(gsb_lib, cuda_device):
     """The synchronous wrapper learns the frame's need from the counts buffer it always hands the library, grows the scratch
     block and renders the frame again inside the call, whether or not the caller asked for the counts."""
     from gs2mesh_b200 import rasterizer as rast
@@ -365,12 +365,9 @@ def test_wrapper_grows_undersized_scratch_and_renders_again(gsb_lib, cuda_device
     ample = _ours(cuda_device, inp)
     need = int(ample["counts"][0])
     assert need > 1024
-    monkeypatch.setattr(rast, "MIN_GUESS", 1024)
-    monkeypatch.setattr(rast, "GUESS_PER_GAUSSIAN", 0)
     for want_counts in (False, True):
-        monkeypatch.setattr(rast, "_scratch", {})  # the first attempt gets a 1024-instance scratch block
-        got = _ours(cuda_device, inp, want_counts=want_counts)
-        (scratch,) = rast._scratch.values()
+        scratch = rast.Scratch(cuda_device, max_instances=1024)  # the first attempt gets a 1024-instance scratch block
+        got = _ours(cuda_device, inp, want_counts=want_counts, scratch=scratch)
         assert scratch.max_instances >= need  # grown, so the frame was rendered again
         for k in ("color", "depth", "final_T", "radii"):
             np.testing.assert_array_equal(got[k], ample[k], err_msg=f"{k} want_counts={want_counts}")

@@ -66,7 +66,7 @@ def _render(case, inp, dev, flags, vt=None, scale_modifier=None):
                                  height=vt.height, shs=inp["shs"], colors_precomp=inp["colors_precomp"], scales=inp["scales"],
                                  rotations=inp["rotations"], cov3D_precomp=inp["cov3D_precomp"], sh_degree=case.sh_degree,
                                  scale_modifier=case.scale_modifier if scale_modifier is None else scale_modifier, flags=flags,
-                                 want_counts=True, **_view(vt, dev))
+                                 want_counts=True, scratch=rast.Scratch(dev), **_view(vt, dev))
     torch.cuda.synchronize()
     return out
 
@@ -199,7 +199,7 @@ def test_cov3d_path_ignores_scale_modifier(oracle, gsb_lib, cuda_device):
     _free()
 
 
-def test_toed_in_pair(oracle, gsb_lib, cuda_device):
+def test_toed_in_pair_in_caller_blocks(oracle, gsb_lib, cuda_device):
     """The fused pair kernel on a convergent rig whose eyes disagree on the near cull and on the frame edges: without a
     shared depth order bit-identical to two single views; claiming a shared depth order raises the flag in both eyes."""
     import torch
@@ -218,32 +218,29 @@ def test_toed_in_pair(oracle, gsb_lib, cuda_device):
     f32 = dict(dtype=torch.float32, device=cuda_device)
     need = max(int(s["counts"][0]) for s in singles)
     streams = (torch.cuda.Stream(cuda_device), torch.cuda.Stream(cuda_device))
-    try:
-        for shared in (False, True):
-            eyes = []
-            for vt in vts:
-                eyes.append(dict(**_view(vt, cuda_device), out_color=torch.empty(3, case.H, case.W, **f32),
-                                 out_depth=torch.empty(case.H, case.W, **f32), out_final_T=torch.empty(case.H, case.W, **f32),
-                                 counts_out=torch.zeros(4, dtype=torch.int64, device=cuda_device)))
-            torch.cuda.synchronize()
-            rast.rasterize_forward_pair(means3D=inp["means3D"], opacities=inp["opacities"], shs=inp["shs"], scales=inp["scales"],
-                                        rotations=inp["rotations"], sh_degree=case.sh_degree, bg=inp["bg"], width=case.W,
-                                        height=case.H, eyes=eyes, streams=streams, flags=rast.DEFAULT_FLAGS, shared_depth=shared,
-                                        min_instances=need)
-            torch.cuda.synchronize()
-            for e, s in zip(eyes, singles):
-                if shared:
-                    assert e["counts_out"][3].item() == 1  # the eyes' view depths differ: the caller must render separately
-                    continue
-                assert e["counts_out"][3].item() == 0
-                assert torch.equal(e["counts_out"][:3], s["counts"][:3])
-                for k, o in (("color", "out_color"), ("depth", "out_depth"), ("final_T", "out_final_T")):
-                    assert torch.equal(e[o], s[k]), k
-            del eyes
-    finally:
-        for key in [k for k in rast._scratch if k[1] in (streams[0].cuda_stream, streams[1].cuda_stream)]:
-            del rast._scratch[key]
-    del singles, inp
+    scratch = (rast.Scratch(cuda_device), rast.Scratch(cuda_device))
+    for shared in (False, True):
+        eyes = []
+        for vt in vts:
+            eyes.append(dict(**_view(vt, cuda_device), out_color=torch.empty(3, case.H, case.W, **f32),
+                             out_depth=torch.empty(case.H, case.W, **f32), out_final_T=torch.empty(case.H, case.W, **f32),
+                             counts_out=torch.zeros(4, dtype=torch.int64, device=cuda_device)))
+        torch.cuda.synchronize()
+        rast.rasterize_forward_pair(means3D=inp["means3D"], opacities=inp["opacities"], shs=inp["shs"], scales=inp["scales"],
+                                    rotations=inp["rotations"], sh_degree=case.sh_degree, bg=inp["bg"], width=case.W,
+                                    height=case.H, eyes=eyes, streams=streams, scratch=scratch, flags=rast.DEFAULT_FLAGS,
+                                    shared_depth=shared, min_instances=need)
+        torch.cuda.synchronize()
+        for e, s in zip(eyes, singles):
+            if shared:
+                assert e["counts_out"][3].item() == 1  # the eyes' view depths differ: the caller must render separately
+                continue
+            assert e["counts_out"][3].item() == 0
+            assert torch.equal(e["counts_out"][:3], s["counts"][:3])
+            for k, o in (("color", "out_color"), ("depth", "out_depth"), ("final_T", "out_final_T")):
+                assert torch.equal(e[o], s[k]), k
+        del eyes
+    del singles, inp, scratch
     _free()
 
 

@@ -69,7 +69,8 @@ def _render(case, inp, dev, flags, vt=None, want_depth=True):
     out = rast.rasterize_forward(means3D=inp["means3D"], opacities=inp["opacities"], viewmatrix=v["viewmatrix"],
                                  projmatrix=v["projmatrix"], campos=v["campos"], bg=inp["bg"], width=vt.width, height=vt.height,
                                  tan_fovx=v["tan_fovx"], tan_fovy=v["tan_fovy"], shs=inp["shs"], scales=inp["scales"],
-                                 rotations=inp["rotations"], sh_degree=0, flags=flags, want_counts=True, want_depth=want_depth)
+                                 rotations=inp["rotations"], sh_degree=0, flags=flags, want_counts=True, want_depth=want_depth,
+                                 scratch=rast.Scratch(dev))
     torch.cuda.synchronize()
     return out
 
@@ -106,16 +107,13 @@ def _within(r, bar, what):
 
 
 def _free():
-    """Drops the rasterizer's cached scratch blocks and torch's cached memory: the cases differ in size by orders of
+    """Drops the case's tensors and scratch blocks and torch's cached memory: the cases differ in size by orders of
     magnitude, and the GPU is shared."""
     import gc
 
     import torch
 
-    from gs2mesh_b200 import rasterizer as rast
-
     gc.collect()
-    rast._scratch.clear()
     torch.cuda.empty_cache()
 
 
@@ -173,7 +171,7 @@ def test_cub_path_is_bit_identical(oracle, gsb_lib, cuda_device, name):
 
 
 @pytest.mark.parametrize("name", PAIR_CASES)
-def test_pair_with_shared_depth_equals_two_views(oracle, gsb_lib, cuda_device, name):
+def test_pair_in_caller_blocks_with_shared_depth_equals_two_views(oracle, gsb_lib, cuda_device, name):
     """rasterize_forward_pair with one depth sort for both eyes (the <16> sort's second gather above 4M Gaussians, a
     3-pass tile sort above 65536 tiles) against two rasterize_forward calls."""
     import torch
@@ -194,20 +192,17 @@ def test_pair_with_shared_depth_equals_two_views(oracle, gsb_lib, cuda_device, n
                          counts_out=torch.zeros(4, dtype=torch.int64, device=cuda_device)))
     streams = (torch.cuda.Stream(cuda_device), torch.cuda.Stream(cuda_device))
     need = max(int(s["counts"][0]) for s in singles)
-    try:
-        torch.cuda.synchronize()
-        rast.rasterize_forward_pair(means3D=inp["means3D"], opacities=inp["opacities"], shs=inp["shs"], scales=inp["scales"],
-                                    rotations=inp["rotations"], sh_degree=0, bg=inp["bg"], width=case.W, height=case.H, eyes=eyes,
-                                    streams=streams, flags=rast.DEFAULT_FLAGS, shared_depth=True, min_instances=need)
-        torch.cuda.synchronize()
-        for e, s in zip(eyes, singles):
-            assert e["counts_out"][3].item() == 0  # the eyes' view depths agree bit for bit
-            assert torch.equal(e["counts_out"][:3], s["counts"][:3])
-            for k, o in (("color", "out_color"), ("depth", "out_depth"), ("final_T", "out_final_T")):
-                assert torch.equal(e[o], s[k]), (name, k)
-    finally:
-        for key in [k for k in rast._scratch if k[1] in (streams[0].cuda_stream, streams[1].cuda_stream)]:
-            del rast._scratch[key]
+    torch.cuda.synchronize()
+    rast.rasterize_forward_pair(means3D=inp["means3D"], opacities=inp["opacities"], shs=inp["shs"], scales=inp["scales"],
+                                rotations=inp["rotations"], sh_degree=0, bg=inp["bg"], width=case.W, height=case.H, eyes=eyes,
+                                streams=streams, scratch=(rast.Scratch(cuda_device), rast.Scratch(cuda_device)),
+                                flags=rast.DEFAULT_FLAGS, shared_depth=True, min_instances=need)
+    torch.cuda.synchronize()
+    for e, s in zip(eyes, singles):
+        assert e["counts_out"][3].item() == 0  # the eyes' view depths agree bit for bit
+        assert torch.equal(e["counts_out"][:3], s["counts"][:3])
+        for k, o in (("color", "out_color"), ("depth", "out_depth"), ("final_T", "out_final_T")):
+            assert torch.equal(e[o], s[k]), (name, k)
     del singles, eyes, inp
     _free()
 
