@@ -12,6 +12,7 @@ _PKG = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_PKG, "libgs2mesh_b200.so")
 
 GSB_OK, GSB_ERR_INVALID, GSB_ERR_WORKSPACE, GSB_ERR_CUDA, GSB_ERR_ALIGNMENT = range(5)
+GSB_PCD_SURFACE, GSB_PCD_VOXELS = 0, 1  # gsb_pcd_* mode
 
 RASTER_EXACT_TILE_CULL = 1
 RASTER_NO_TMA = 2
@@ -93,6 +94,9 @@ SIGNATURES = {
     "gsb_mesh_clusters": (C.c_int, [_vp, C.c_int64, C.c_int64, _vp, _vp, C.c_size_t, _vp, _vp, _vp, _vp, _vp]),
     "gsb_mesh_remove_small_clusters": (C.c_int, [_vp, C.c_int64, C.c_int64, _vp, _vp, C.c_double, _vp, C.c_size_t, _vp, _vp,
                                                  _vp, _vp]),
+    "gsb_pcd_count": (C.c_int, [_vp, C.POINTER(C.c_int32), _vp, C.c_uint32, C.c_int, _vp, _vp]),
+    "gsb_pcd_emit": (C.c_int, [_vp, C.POINTER(C.c_int32), _vp, C.c_uint32, C.c_int, _vp, _vp, _vp]),
+    "gsb_pcd_points": (C.c_int, [_vp, C.POINTER(C.c_int32), _vp, C.c_int64, C.c_int, _vp, _vp, _vp, _vp]),
     "gsb_eval_sample_count": (C.c_int, [_vp, C.c_int64, _vp, C.c_int64, C.c_double, _vp, _vp]),
     "gsb_eval_sample_emit": (C.c_int, [_vp, C.c_int64, _vp, C.c_int64, C.c_double, _vp, _vp, _vp]),
     "gsb_eval_grid_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int64]),

@@ -240,3 +240,87 @@ def extract_triangle_mesh(volume, with_colors: Optional[bool] = None) -> Triangl
         mesh.edge_keys = uniq.cpu().numpy()  # (voxel index inside `key_window` * 3 + axis) per vertex, for tests
         mesh.key_window = (tuple(int(v) for v in lo), tuple(int(v) for v in (hi - lo + 2)))  # (brick origin, brick count)
     return mesh
+
+
+class PointCloud:
+    """Minimal stand-in for open3d.geometry.PointCloud: fp64 points, colours and normals as host arrays (None when
+    absent)."""
+
+    def __init__(self, points, colors=None, normals=None, device=None):
+        self.device = None if device is None else torch.device(device)
+        self.points = np.asarray(points, dtype=np.float64).reshape(-1, 3)
+        self.colors = None if colors is None else np.asarray(colors, dtype=np.float64).reshape(-1, 3)
+        self.normals = None if normals is None else np.asarray(normals, dtype=np.float64).reshape(-1, 3)
+
+    # Open3D: non-empty, one entry per point
+    def has_colors(self):
+        return len(self.points) > 0 and self.colors is not None and len(self.colors) == len(self.points)
+
+    def has_normals(self):
+        return len(self.points) > 0 and self.normals is not None and len(self.normals) == len(self.points)
+
+    def scale(self, scale, center=(0, 0, 0)):
+        c = np.asarray(center, dtype=np.float64)
+        self.points = (self.points - c) * float(scale) + c
+        return self
+
+    # -- o3d.io.write_point_cloud(path, pcd): binary little-endian PLY, double coordinates and normals, uchar colours
+    def write_ply(self, path):
+        from .io import write_point_cloud_ply
+
+        return write_point_cloud_ply(path, self.points, self.colors, self.normals)
+
+
+def _extract_cloud(volume, mode, with_colors, with_normals):
+    """The sorted keys of `volume`'s cloud and their attributes: count -> scan -> emit -> sort -> points."""
+    dev = volume.device
+    L = _lib.lib()
+    empty = lambda on: np.zeros((0, 3)) if on else None
+    with torch.cuda.device(dev):
+        stream = _lib.stream(dev)
+        nb = volume.num_bricks()  # every brick ever opened = pool slots [0, nb)
+        if nb == 0:
+            return PointCloud(np.zeros((0, 3)), empty(with_colors), empty(with_normals), device=dev)
+        bricks = torch.arange(nb, dtype=torch.int32, device=dev)
+        # the key window of extract_triangle_mesh: the bounding box of the open bricks and their +1 neighbours
+        idx = volume._index[:nb, :3]
+        lo = idx.min(dim=0).values.cpu().numpy().astype(np.int64)
+        hi = idx.max(dim=0).values.cpu().numpy().astype(np.int64)
+        window = (C.c_int32 * 6)(*[int(v) for v in lo], *[int(v) for v in (hi - lo + 2)])
+        counts = torch.zeros(nb, dtype=torch.int32, device=dev)
+        _lib.check(L.gsb_pcd_count(volume._h, window, ptr(bricks), nb, mode, ptr(counts), stream))
+        offsets = torch.cumsum(counts.to(torch.int64), 0) - counts.to(torch.int64)
+        n = int(counts.sum().item())
+        key_window = (tuple(int(v) for v in lo), tuple(int(v) for v in (hi - lo + 2)))
+        if n == 0:
+            pcd = PointCloud(np.zeros((0, 3)), empty(with_colors), empty(with_normals), device=dev)
+            pcd.keys, pcd.key_window = np.zeros(0, np.int64), key_window
+            return pcd
+        keys = torch.empty(n, dtype=torch.int64, device=dev)
+        _lib.check(L.gsb_pcd_emit(volume._h, window, ptr(bricks), nb, mode, ptr(offsets.contiguous()), ptr(keys), stream))
+        keys = torch.sort(keys).values  # every key has one owner brick: no duplicates to remove
+        xyz = torch.empty(n, 3, dtype=torch.float64, device=dev)
+        rgb = torch.empty(n, 3, dtype=torch.float64, device=dev) if with_colors else None
+        nrm = torch.empty(n, 3, dtype=torch.float64, device=dev) if with_normals else None
+        _lib.check(L.gsb_pcd_points(volume._h, window, ptr(keys), n, mode, ptr(xyz), ptr(rgb), ptr(nrm), stream))
+        host = lambda t: None if t is None else t.cpu().numpy()
+        pcd = PointCloud(host(xyz), host(rgb), host(nrm), device=dev)
+        pcd.keys = keys.cpu().numpy()  # window voxel index (* 3 + axis for the surface cloud) per point, for tests
+        pcd.key_window = key_window  # (brick origin, brick count)
+    return pcd
+
+
+def extract_point_cloud(volume, with_colors: Optional[bool] = None, with_normals: bool = True) -> PointCloud:
+    """`volume.extract_point_cloud()` for a gs2mesh_b200.tsdf.TSDFVolume: Open3D's ScalableTSDFVolume::ExtractPointCloud,
+    the zero crossings of the TSDF along the lattice axes with interpolated colours and TSDF-gradient normals, in
+    ascending edge key (window voxel index * 3 + axis)."""
+    with_colors = (volume.color is not None) if with_colors is None else bool(with_colors)
+    if with_colors and volume.color is None:
+        raise ValueError("extract_point_cloud: the volume has no colour")
+    return _extract_cloud(volume, _lib.GSB_PCD_SURFACE, with_colors, bool(with_normals))
+
+
+def extract_voxel_point_cloud(volume) -> PointCloud:
+    """`volume.extract_voxel_point_cloud()`: Open3D's ScalableTSDFVolume::ExtractVoxelPointCloud, the centre of every
+    voxel with weight != 0 and -0.98 <= tsdf < 0.98, grey (tsdf + 1) / 2, in ascending window voxel index."""
+    return _extract_cloud(volume, _lib.GSB_PCD_VOXELS, True, False)

@@ -13,6 +13,12 @@ gs2mesh_utils/tsdf_utils.py touches, so its body (lines 51-142) reads the same w
     clusters, n_tri, area = mesh.cluster_connected_triangles(); mesh.remove_triangles_by_mask(mask);
     mesh.remove_unreferenced_vertices()                                                                          # :132-140
 
+and Open3D's other two read-outs of the volume, which the evaluators take as input:
+
+    pcd = volume.extract_point_cloud()          # geometry.PointCloud: points, colors, normals; has_colors(), has_normals()
+    vox = volume.extract_voxel_point_cloud()    # voxel centres near the surface, grey by tsdf
+    o3d.io.write_point_cloud(path, pcd)
+
 Differences from Open3D, by construction: the volume lives in GPU memory (an unbounded, hashed set of 16^3 bricks on
 the same voxel lattice, like Open3D's; `window_resolution=` only sets the window dense read-backs look at); images are uploaded on
 integrate().  Everything else (argument names, the RuntimeError on mismatching image sizes, float32 depth
@@ -25,8 +31,11 @@ from types import SimpleNamespace
 
 import numpy as np
 
+from .mesh import PointCloud as _PointCloud
 from .mesh import TriangleMesh as _Mesh
+from .mesh import extract_point_cloud as _extract_pcd
 from .mesh import extract_triangle_mesh as _extract
+from .mesh import extract_voxel_point_cloud as _extract_voxel_pcd
 
 
 class Image:
@@ -139,12 +148,29 @@ class ScalableTSDFVolume:
         m = _extract(self._vol)
         return TriangleMesh(m.vertices, m.triangles, m.vertex_colors, m.vertex_normals, device=m.device)
 
+    def extract_point_cloud(self):
+        p = _extract_pcd(self._vol)
+        return PointCloud(p.points, p.colors, p.normals, device=p.device)
+
+    def extract_voxel_point_cloud(self):
+        p = _extract_voxel_pcd(self._vol)
+        return PointCloud(p.points, p.colors, p.normals, device=p.device)
+
     def reset(self):
         self._vol.reset()
 
 
+class PointCloud(_PointCloud):
+    """open3d.geometry.PointCloud: points, colors, normals (fp64 host arrays), has_colors(), has_normals()."""
+
+
 def _write_triangle_mesh(path, mesh, **_):
     mesh.write_ply(path)
+    return True
+
+
+def _write_point_cloud(path, pointcloud, **_):
+    pointcloud.write_ply(path)
     return True
 
 
@@ -154,9 +180,9 @@ def _verbosity(_level):
 
 
 # module tree mirroring `open3d`
-geometry = SimpleNamespace(Image=Image, RGBDImage=RGBDImage, TriangleMesh=TriangleMesh)
+geometry = SimpleNamespace(Image=Image, RGBDImage=RGBDImage, TriangleMesh=TriangleMesh, PointCloud=PointCloud)
 camera = SimpleNamespace(PinholeCameraIntrinsic=PinholeCameraIntrinsic)
 pipelines = SimpleNamespace(integration=SimpleNamespace(ScalableTSDFVolume=ScalableTSDFVolume, TSDFVolumeColorType=TSDFVolumeColorType))
-io = SimpleNamespace(write_triangle_mesh=_write_triangle_mesh)
+io = SimpleNamespace(write_triangle_mesh=_write_triangle_mesh, write_point_cloud=_write_point_cloud)
 utility = SimpleNamespace(VerbosityContextManager=_verbosity, VerbosityLevel=SimpleNamespace(Debug=0, Info=1, Warning=2, Error=3))
 __version__ = "0.17.0-gs2mesh_b200"

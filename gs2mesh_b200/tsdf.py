@@ -557,6 +557,15 @@ class TSDF:
         self.mesh.compute_vertex_normals(self.volume.device)
         return self.mesh
 
+    def extract_point_cloud(self):
+        """`volume.extract_point_cloud()` scaled by TSDF_scale about the origin, like the mesh: the surface cloud in
+        world units, with colours and TSDF-gradient normals."""
+        from .mesh import extract_point_cloud
+
+        if self.volume is None:
+            raise RuntimeError("TSDF.extract_point_cloud() called before run()/integrate()")
+        return extract_point_cloud(self.volume).scale(float(self._arg("TSDF_scale", 1.0)), (0, 0, 0))
+
     def save_mesh(self):
         """tsdf_utils.py:112-120"""
         if self.mesh is None:

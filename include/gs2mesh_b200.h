@@ -356,6 +356,31 @@ int gsb_mesh_remove_small_clusters(const int64_t* triangles, int64_t n_triangles
                                    int64_t* out_triangles, int64_t* vertex_ids, int64_t* sizes, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Point clouds: volume.extract_point_cloud() / extract_voxel_point_cloud()
+ * (Open3D ScalableTSDFVolume::ExtractPointCloud / ExtractVoxelPointCloud; DESIGN.md section 7, "Point clouds")
+ * ------------------------------------------------------------------------------------------
+ * `mode` picks the cloud.  GSB_PCD_SURFACE: one point per lattice edge from a voxel to its +1 neighbour on one axis
+ * where both voxels have weight != 0 and -0.98f <= tsdf < 0.98f and the float product of their tsdf is < 0 (a
+ * neighbour in a brick that was never opened has weight 0).  GSB_PCD_VOXELS: one point per voxel with weight != 0 and
+ * -0.98f <= tsdf < 0.98f.  bricks and window are those of gsb_mesh_count; points are identified by a key =
+ * ((gx*NY + gy)*NZ + gz)*3 + axis (surface) or (gx*NY + gy)*NZ + gz (voxels) over the voxel grid of `window`, which
+ * must fit 63 bits like the mesh's edge keys, otherwise GSB_ERR_INVALID.  Every key has exactly one owner brick, so the
+ * keys need no de-duplication; the caller sorts them (the cloud's order is ascending key).
+ *   gsb_pcd_count   counts[b] = points of brick b (device uint32[n_bricks])
+ *   gsb_pcd_emit    the keys of brick b at keys[offsets[b]...] (device int64), in no particular order inside a brick
+ *   gsb_pcd_points  n keys -> xyz (device double [n,3]), rgb (device double [n,3] or NULL) and normals (device double
+ *                   [n,3] or NULL; GSB_PCD_SURFACE only), equal to Open3D's doubles (one rounding per operation in its
+ *                   order).  Surface rgb needs a volume with colour; the voxel cloud's rgb is the grey (tsdf + 1) / 2. */
+#define GSB_PCD_SURFACE 0
+#define GSB_PCD_VOXELS 1
+int gsb_pcd_count(const GsbVolume* vol, const int32_t* window, const uint32_t* bricks, uint32_t n_bricks, int mode,
+                  uint32_t* counts, void* stream);
+int gsb_pcd_emit(const GsbVolume* vol, const int32_t* window, const uint32_t* bricks, uint32_t n_bricks, int mode,
+                 const int64_t* offsets, int64_t* keys, void* stream);
+int gsb_pcd_points(const GsbVolume* vol, const int32_t* window, const int64_t* keys, int64_t n, int mode, double* xyz,
+                   double* rgb, double* normals, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Mesh-quality evaluation (evaluation/DTU/eval_code/eval.py, MobileBrick evaluate.py) without Open3D / sklearn.
  * All arithmetic is fp64 with explicit roundings (no FMA contraction), in the reference's operation order.
  * ------------------------------------------------------------------------------------------
