@@ -97,6 +97,8 @@ SIGNATURES = {
     "gsb_pcd_count": (C.c_int, [_vp, C.POINTER(C.c_int32), _vp, C.c_uint32, C.c_int, _vp, _vp]),
     "gsb_pcd_emit": (C.c_int, [_vp, C.POINTER(C.c_int32), _vp, C.c_uint32, C.c_int, _vp, _vp, _vp]),
     "gsb_pcd_points": (C.c_int, [_vp, C.POINTER(C.c_int32), _vp, C.c_int64, C.c_int, _vp, _vp, _vp, _vp]),
+    "gsb_tsdf_raycast": (C.c_int, [_vp, C.c_int32, C.c_int32, C.c_double, C.c_double, C.c_double, C.c_double,
+                                   C.POINTER(C.c_double), C.c_double, C.c_double, _vp, _vp, _vp, _vp]),
     "gsb_eval_sample_count": (C.c_int, [_vp, C.c_int64, _vp, C.c_int64, C.c_double, _vp, _vp]),
     "gsb_eval_sample_emit": (C.c_int, [_vp, C.c_int64, _vp, C.c_int64, C.c_double, _vp, _vp, _vp]),
     "gsb_eval_grid_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int64]),

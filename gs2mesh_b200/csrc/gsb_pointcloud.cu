@@ -78,44 +78,6 @@ __global__ void __launch_bounds__(256) pcd_brick_kernel(const VolView v, const u
   if (!offsets && threadIdx.x == 0) counts[blockIdx.x] = s_count;
 }
 
-// ScalableTSDFVolume::GetTSDFAt(p) in double, one rounding per operation: the unit of p - vl/2, the cube of voxels
-// around it (clamped into the unit; corners past 15 step into the +1 units), trilinear weights from the fractional
-// grid position.  A missing unit gives 0.0 for the whole sample, a missing +1 unit 0 for its corners; weights are not
-// consulted.
-__device__ double tsdf_at(const VolView& v, double vl, double U, double half, const double p[3]) {
-  int i0[3], c[3];
-  double q[3], r[3];
-#pragma unroll
-  for (int k = 0; k < 3; ++k) {
-    q[k] = __dsub_rn(p[k], half);
-    i0[k] = (int)floor(__ddiv_rn(q[k], U));
-  }
-  const uint32_t s0 = slot_of_brick(v, i0[0], i0[1], i0[2]);
-  if (s0 == kSlotNone) return 0.0;
-#pragma unroll
-  for (int k = 0; k < 3; ++k) {
-    const double g = __ddiv_rn(__dsub_rn(q[k], __dmul_rn((double)i0[k], U)), vl);
-    c[k] = min(max((int)floor(g), 0), GSB_BRICK - 1);
-    r[k] = __dsub_rn(g, (double)c[k]);
-  }
-  // corners in kMcShift order: (0,0,0) (1,0,0) (1,1,0) (0,1,0) (0,0,1) (1,0,1) (1,1,1) (0,1,1)
-  constexpr int sx[8] = {0, 1, 1, 0, 0, 1, 1, 0}, sy[8] = {0, 0, 1, 1, 0, 0, 1, 1}, sz[8] = {0, 0, 0, 0, 1, 1, 1, 1};
-  double f[8];
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    const int x = c[0] + sx[i], y = c[1] + sy[i], z = c[2] + sz[i];
-    const uint32_t slot = (x | y | z) < GSB_BRICK ? s0 : slot_of_brick(v, i0[0] + (x >> 4), i0[1] + (y >> 4), i0[2] + (z >> 4));
-    f[i] = slot == kSlotNone ? 0.0
-                             : (double)v.tw[(size_t)slot * GSB_BRICK_VOXELS + ((x & 15) * 16 + (y & 15)) * 16 + (z & 15)].x;
-  }
-  const double a0 = __dsub_rn(1.0, r[0]), a1 = __dsub_rn(1.0, r[1]), a2 = __dsub_rn(1.0, r[2]);
-  const double lo = __dadd_rn(__dmul_rn(a1, __dadd_rn(__dmul_rn(a2, f[0]), __dmul_rn(r[2], f[4]))),
-                              __dmul_rn(r[1], __dadd_rn(__dmul_rn(a2, f[3]), __dmul_rn(r[2], f[7]))));
-  const double hi = __dadd_rn(__dmul_rn(a1, __dadd_rn(__dmul_rn(a2, f[1]), __dmul_rn(r[2], f[5]))),
-                              __dmul_rn(r[1], __dadd_rn(__dmul_rn(a2, f[2]), __dmul_rn(r[2], f[6]))));
-  return __dadd_rn(__dmul_rn(a0, lo), __dmul_rn(r[0], hi));
-}
-
 // One sorted key -> point, colour and normal.  Surface cloud (ExtractPointCloud), for the edge from voxel (x,y,z) of
 // unit index0 to its +1 neighbour on `axis`:
 //   p0 = (vl/2 + vl*x, vl/2 + vl*y, vl/2 + vl*z) + index0 * U    (per unit, not vl/2 + vl*(16*b + x))
@@ -172,21 +134,8 @@ __global__ void __launch_bounds__(256) pcd_points_kernel(const VolView v, const 
       rgb[3 * i + k] = (double)__fdiv_rn(__fdiv_rn(__fadd_rn(__fmul_rn(k0[k], r1), __fmul_rn(k1[k], r0)), rs), 255.0f);
   }
   if (normals) {
-    const double h = __dmul_rn(0.99, vl);
     double nv[3];
-#pragma unroll 1
-    for (int j = 0; j < 3; ++j) {
-      double pm[3] = {p[0], p[1], p[2]}, pp[3] = {p[0], p[1], p[2]};
-      pm[j] = __dsub_rn(pm[j], h);
-      pp[j] = __dadd_rn(pp[j], h);
-      nv[j] = __dsub_rn(tsdf_at(v, vl, U, half, pp), tsdf_at(v, vl, U, half, pm));
-    }
-    const double sq = __dadd_rn(__dadd_rn(__dmul_rn(nv[0], nv[0]), __dmul_rn(nv[1], nv[1])), __dmul_rn(nv[2], nv[2]));
-    if (sq > 0.0) {
-      const double len = __dsqrt_rn(sq);
-#pragma unroll
-      for (int j = 0; j < 3; ++j) nv[j] = __ddiv_rn(nv[j], len);
-    }
+    tsdf_normal(v, vl, U, half, p, nv);
 #pragma unroll
     for (int j = 0; j < 3; ++j) normals[3 * i + j] = nv[j];
   }

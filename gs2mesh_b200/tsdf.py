@@ -17,7 +17,7 @@ from __future__ import annotations
 
 import ctypes as C
 import os
-from typing import Optional, Sequence
+from typing import NamedTuple, Optional, Sequence
 
 import numpy as np
 import torch
@@ -32,6 +32,14 @@ def default_window(resolution: int = 512):
     (`TSDFVolume.bricks()` / `.dense()`): the volume itself is unbounded."""
     nb = resolution // BRICK
     return (-(nb // 2),) * 3, (nb,) * 3
+
+
+class RayCast(NamedTuple):
+    """Images of a ray cast, device float32: depth [H,W] (0 where the ray hit nothing), normals [H,W,3] in world
+    coordinates and colours [H,W,3] in [0,1] (zero without a hit; None when not asked for)."""
+    depth: torch.Tensor
+    normals: Optional[torch.Tensor]
+    colors: Optional[torch.Tensor]
 
 
 DEFAULT_POOL_BRICKS = 1 << 15  # 32768 bricks = 1 GiB of (tsdf, weight) + 2 GiB of colour; grown on demand
@@ -319,6 +327,27 @@ class TSDFVolume:
         self._counters.zero_()
         self.frames_integrated = 0
 
+    # ------------------------------------------------------------------ ray casting
+    def raycast(self, width, height, fx, fy, cx, cy, extrinsic_w2c, depth_min, depth_max, *, normals=True, colors=None):
+        """Depth, normal and colour images of the fused surface seen by a pinhole camera (`gsb_tsdf_raycast`,
+        include/gs2mesh_b200.h), in volume units: extrinsic_w2c = 4x4 world->camera (host), depth = camera-frame z of the
+        first entry into the surface within [depth_min, depth_max].  colors=None gives colours when the volume keeps
+        them; colors=True on a volume without colour raises ValueError."""
+        if colors is None:
+            colors = self.color is not None
+        if colors and self.color is None:
+            raise ValueError("raycast: colours asked of a volume without colour (with_color=False)")
+        w, h = int(width), int(height)
+        e = np.ascontiguousarray(np.asarray(extrinsic_w2c, dtype=np.float64).reshape(16))
+        depth = torch.empty(h, w, dtype=torch.float32, device=self.device)
+        nrm = torch.empty(h, w, 3, dtype=torch.float32, device=self.device) if normals else None
+        col = torch.empty(h, w, 3, dtype=torch.float32, device=self.device) if colors else None
+        with torch.cuda.device(self.device):
+            _lib.check(self._L.gsb_tsdf_raycast(self._h, w, h, float(fx), float(fy), float(cx), float(cy),
+                                                e.ctypes.data_as(C.POINTER(C.c_double)), float(depth_min), float(depth_max),
+                                                ptr(depth), ptr(nrm), ptr(col), self._stream()), invalid_is_value_error=True)
+        return RayCast(depth, nrm, col)
+
     # ------------------------------------------------------------------ multi-GPU merge
     def to_sums(self):
         with torch.cuda.device(self.device):
@@ -504,14 +533,37 @@ class TSDF:
         scale = float(self._arg("TSDF_scale", 1.0))
         baseline = float(self.renderer.baseline)
         w, h = int(left_camera["width"]), int(left_camera["height"])
-        extrinsic = np.array(left_camera["extrinsic"], dtype=np.float64).copy()
-        extrinsic[:3, 3] /= scale  # tsdf_utils.py:85-86
         prepared = self.volume.prepare_depth(
             depth, w, h, final_T=final_T, mask=mask,
             min_depth=float(self._arg("TSDF_min_depth_baselines", 4)) * baseline,  # :83
             depth_scale=scale, depth_trunc=baseline * float(self._arg("TSDF_max_depth_baselines", 20)) / scale)  # :92
         self.volume.integrate(prepared, rgb, w, h, left_camera["fx"], left_camera["fy"], left_camera["cx"],
-                              left_camera["cy"], np.linalg.inv(extrinsic))  # :106-107
+                              left_camera["cy"], self._world_to_camera(left_camera))  # :106-107
+
+    def _world_to_camera(self, camera):
+        """The volume-unit world->camera matrix integrate passes for a camera dict: translation / TSDF_scale, then
+        inverted (tsdf_utils.py:85-86, :106)."""
+        extrinsic = np.array(camera["extrinsic"], dtype=np.float64).copy()
+        extrinsic[:3, 3] /= float(self._arg("TSDF_scale", 1.0))
+        return np.linalg.inv(extrinsic)
+
+    def raycast(self, camera, depth_range=None, *, normals=True, colors=None):
+        """Ray-cast the fused volume from a camera dict of the shape `Renderer.left_cameras` holds: depth in world units
+        (the volume's depth times TSDF_scale, 0 where nothing was hit) on that camera's pixel grid, world-frame normals and
+        colours in [0,1] (TSDFVolume.raycast).  depth_range = (near, far) in world units; the default is the range
+        integrate keeps, [TSDF_min_depth_baselines, TSDF_max_depth_baselines] baselines.  Cast from a view's left camera,
+        the depth lies on the pixel grid of that view's stereo depth, so the two can be subtracted."""
+        if self.volume is None:
+            raise RuntimeError("TSDF.raycast() called before run()/integrate()")
+        scale = float(self._arg("TSDF_scale", 1.0))
+        if depth_range is None:
+            baseline = float(self.renderer.baseline)
+            depth_range = (float(self._arg("TSDF_min_depth_baselines", 4)) * baseline,
+                           float(self._arg("TSDF_max_depth_baselines", 20)) * baseline)
+        out = self.volume.raycast(int(camera["width"]), int(camera["height"]), camera["fx"], camera["fy"], camera["cx"],
+                                  camera["cy"], self._world_to_camera(camera), depth_range[0] / scale,
+                                  depth_range[1] / scale, normals=normals, colors=colors)
+        return out._replace(depth=out.depth * scale)
 
     def run(self, visualize=False, views: Optional[Sequence[int]] = None):
         """tsdf_utils.py:39-110.  `views` restricts the loop (used for view sharding across ranks).  The volume is unbounded

@@ -381,6 +381,34 @@ int gsb_pcd_points(const GsbVolume* vol, const int32_t* window, const int64_t* k
                    double* rgb, double* normals, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Ray casting: the depth, normal and colour images of the fused zero-level surface seen by one pinhole camera
+ * (DESIGN.md section 7, "Ray casting"; KinectFusion's read-out, defined here since ScalableTSDFVolume has none)
+ * ------------------------------------------------------------------------------------------
+ * Pixel (u,v) (integers: the pixel integrate assigns to camera points with x fx/z + cx in [u - 0.5, u + 0.5)) casts the
+ * ray p(z) = o + z d, o = -R^T t, d = R^T ((u - cx)/fx, (v - cy)/fy, 1), with [R|t] = extrinsic_w2c (host, row-major
+ * double[16]); z is the camera-frame depth, comparable with the integrated depth image.  A sample at p takes
+ * GetTSDFAt's cube (the unit of p - vl/2, the base voxel clamped into it, corners past 15 in the +1 units) and is
+ *   EMPTY   if that unit is not open or lies outside the lattice range [-2^20, 2^20),
+ *   INVALID if any of the 8 corners has weight 0 (a corner in an unopened unit counts as weight 0: the mesh's rule),
+ *   VALID   otherwise, with f = GetTSDFAt(p).
+ * The march runs from z = max(depth_min, entry into the lattice box) while z <= min(depth_max, exit from it), and
+ * steps to the exit from an EMPTY unit's box, by vl/|d| after an INVALID or a VALID sample with f <= 0, and by
+ * max(f * sdf_trunc, vl)/|d| after a VALID f > 0.  Two consecutive VALID samples with f_prev > 0 >= f are the hit
+ * z* = z_prev + (z - z_prev) * (f_prev / (f_prev - f)) (back faces give none).  At a hit, all fp64 and rounded once:
+ *   depth   (float)z*                                                     device float [H,W] (required)
+ *   normals GetNormalAt(p*).normalized(), world coordinates (the surface
+ *           point cloud's formula)                                        device float [H,W,3] or NULL
+ *   colors  the trilinear interpolation of the stored colour over the
+ *           cube of p* (weights not read) / 255, in [0,1]                 device float [H,W,3] or NULL
+ * A ray without a hit gets depth 0 and zero normal and colour.  GSB_ERR_INVALID, before any launch, for
+ * 1 <= width <= GSB_TSDF_MAX_WIDTH / 1 <= height <= GSB_TSDF_MAX_HEIGHT violated, fx or fy <= 0, a non-finite intrinsic,
+ * extrinsic entry or depth bound, !(0 <= depth_min < depth_max), or colors asked of a volume without colour.
+ * Enqueued on `stream`; allocates nothing.  Each ray's cost grows with the units and unobserved voxels it crosses. */
+int gsb_tsdf_raycast(const GsbVolume* vol, int32_t width, int32_t height, double fx, double fy, double cx, double cy,
+                     const double* extrinsic_w2c, double depth_min, double depth_max, float* depth, float* normals,
+                     float* colors, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Mesh-quality evaluation (evaluation/DTU/eval_code/eval.py, MobileBrick evaluate.py) without Open3D / sklearn.
  * All arithmetic is fp64 with explicit roundings (no FMA contraction), in the reference's operation order.
  * ------------------------------------------------------------------------------------------
