@@ -9,6 +9,9 @@
 // in shared memory; a count pass and an emit pass write three 64-bit edge keys per triangle
 // (key = global voxel index * 3 + axis); the caller uniques the keys (vertex ids) and a vertex
 // kernel evaluates positions / colours per unique edge in fp64 with Open3D's formulas.
+// Triangle order: the caller lists the bricks in ascending lattice index; the emit pass places a brick's triangles by a
+// block-wide scan of the per-cube counts, so cubes follow in pool-layout order x*256 + y*16 + z and each cube's triangles
+// in the case table's order.  The mesh therefore does not depend on pool order or on warp scheduling.
 //
 // Cluster cleaning (tsdf_utils.py:122-142, TriangleMesh::ClusterConnectedTriangles + removal of small clusters and
 // unreferenced vertices): triangles sharing an edge are grouped by a radix sort of 64-bit edge keys, joined by a
@@ -39,14 +42,19 @@ __device__ __forceinline__ int cube_case(const float2* s, int x, int y, int z) {
   return c == 255 ? 0 : c;
 }
 
-// mode 0: tri_counts[b] = number of triangles of brick b.  mode 1: write the edge keys.
-__global__ void __launch_bounds__(256) mc_brick_kernel(const VolView v, const uint32_t* __restrict__ bricks, int mode,
-                                                       uint32_t* __restrict__ tri_counts,
-                                                       const long long* __restrict__ tri_offsets,
-                                                       long long* __restrict__ edge_keys) {
+constexpr int kMcThreads = 256;
+using McScan = cub::BlockScan<uint32_t, kMcThreads>;
+
+// mode 0: tri_counts[b] = number of triangles of brick b.  mode 1: write the edge keys, cube i's triangles after those of
+// cubes 0 .. i-1 of the brick.  Launched with kMcThreads threads: each of the 16 rounds covers cubes [256k, 256k + 256).
+__global__ void __launch_bounds__(kMcThreads) mc_brick_kernel(const VolView v, const uint32_t* __restrict__ bricks, int mode,
+                                                              uint32_t* __restrict__ tri_counts,
+                                                              const long long* __restrict__ tri_offsets,
+                                                              long long* __restrict__ edge_keys) {
   __shared__ float2 s[kHalo * kHalo * kHalo];
   __shared__ uint32_t s_count;
   __shared__ uint32_t s_nb[8];  // pool slots of the brick and its +1 neighbours (bit 2: x+1, bit 1: y+1, bit 0: z+1)
+  __shared__ McScan::TempStorage s_scan;
   const uint32_t brick = bricks[blockIdx.x];
   const int4 bi = v.index[brick];
   // window-relative brick coordinates (the edge keys are relative to the key window)
@@ -64,16 +72,18 @@ __global__ void __launch_bounds__(256) mc_brick_kernel(const VolView v, const ui
                              : v.tw[(size_t)slot * GSB_BRICK_VOXELS + ((x & 15) * 16 + (y & 15)) * 16 + (z & 15)];
   }
   __syncthreads();
-  const long long base = mode ? tri_offsets[blockIdx.x] : 0;
+  long long base = mode ? tri_offsets[blockIdx.x] : 0;  // emit: where this round's first triangle goes
   const long long NY = (long long)v.nb[1] * GSB_BRICK, NZ = (long long)v.nb[2] * GSB_BRICK;
-  for (int i = threadIdx.x; i < GSB_BRICK_VOXELS; i += blockDim.x) {
+  for (int i = threadIdx.x; i < GSB_BRICK_VOXELS; i += kMcThreads) {
     const int z = i & 15, y = (i >> 4) & 15, x = i >> 8;
     const int c = cube_case(s, x, y, z);
-    if (c == 0) continue;
     int ntri = 0;
     while (ntri < 5 && kMcTriTable[c][3 * ntri] >= 0) ++ntri;
-    const uint32_t slot = atomicAdd(&s_count, (uint32_t)ntri);
-    if (mode) {
+    if (mode == 0) {
+      if (ntri) atomicAdd(&s_count, (uint32_t)ntri);  // an integer sum: the same whatever the order
+    } else {
+      uint32_t slot, round_total;
+      McScan(s_scan).ExclusiveSum((uint32_t)ntri, slot, round_total);
       for (int t = 0; t < ntri; ++t) {
         // Open3D pushes (e0, e2, e1): ScalableTSDFVolume.cpp ExtractTriangleMesh
         const int order[3] = {0, 2, 1};
@@ -85,6 +95,8 @@ __global__ void __launch_bounds__(256) mc_brick_kernel(const VolView v, const ui
           edge_keys[3 * (base + slot + t) + k] = ((gx * NY + gy) * NZ + gz) * 3 + kMcEdgeShift[e][3];
         }
       }
+      base += round_total;
+      __syncthreads();  // s_scan is reused by the next round
     }
   }
   __syncthreads();
@@ -435,7 +447,7 @@ int gsb_mesh_count(const GsbVolume* vol, const int32_t* window, const uint32_t* 
   if (!vol || (n_bricks && (!bricks || !tri_counts))) return fail(GSB_ERR_INVALID, "mesh_count: bad arguments");
   if (const int rc = window_check("mesh_count", window)) return rc;
   if (n_bricks == 0) return GSB_OK;
-  mc_brick_kernel<<<n_bricks, 256, 0, stream>>>(view_of(vol, window), bricks, 0, tri_counts, nullptr, nullptr);
+  mc_brick_kernel<<<n_bricks, kMcThreads, 0, stream>>>(view_of(vol, window), bricks, 0, tri_counts, nullptr, nullptr);
   count_launch();
   return check_launch("mc_brick_kernel(count)", stream, false);
 }
@@ -446,7 +458,7 @@ int gsb_mesh_emit(const GsbVolume* vol, const int32_t* window, const uint32_t* b
   if (!vol || (n_bricks && (!bricks || !tri_offsets || !edge_keys))) return fail(GSB_ERR_INVALID, "mesh_emit: bad arguments");
   if (const int rc = window_check("mesh_emit", window)) return rc;
   if (n_bricks == 0) return GSB_OK;
-  mc_brick_kernel<<<n_bricks, 256, 0, stream>>>(view_of(vol, window), bricks, 1, nullptr, reinterpret_cast<const long long*>(tri_offsets),
+  mc_brick_kernel<<<n_bricks, kMcThreads, 0, stream>>>(view_of(vol, window), bricks, 1, nullptr, reinterpret_cast<const long long*>(tri_offsets),
                                                 reinterpret_cast<long long*>(edge_keys));
   count_launch();
   return check_launch("mc_brick_kernel(emit)", stream, false);

@@ -205,7 +205,9 @@ def remove_vertices_by_mask(vertices, triangles, vertex_mask, vertex_colors=None
 
 
 def extract_triangle_mesh(volume, with_colors: Optional[bool] = None) -> TriangleMesh:
-    """`volume.extract_triangle_mesh()` for a gs2mesh_b200.tsdf.TSDFVolume."""
+    """`volume.extract_triangle_mesh()` for a gs2mesh_b200.tsdf.TSDFVolume.  Vertices are in ascending edge key; triangles
+    in Open3D's loop order with the volume units visited in lattice order: bricks in ascending lattice index (bx, by, bz),
+    inside a brick cubes in pool-layout order x*256 + y*16 + z, inside a cube the case table's triangles."""
     dev = volume.device
     L = _lib.lib()
     with_colors = (volume.color is not None) if with_colors is None else with_colors
@@ -215,12 +217,16 @@ def extract_triangle_mesh(volume, with_colors: Optional[bool] = None) -> Triangl
         if nb == 0:
             return TriangleMesh(np.zeros((0, 3)), np.zeros((0, 3), np.int64), np.zeros((0, 3)) if with_colors else None,
                                 device=dev)
-        bricks = torch.arange(nb, dtype=torch.int32, device=dev)
         # edge keys are voxel indices inside the bounding box of the open bricks (+1: a cube reaches into its +1 neighbours)
-        idx = volume._index[:nb, :3]
-        lo = idx.min(dim=0).values.cpu().numpy().astype(np.int64)
-        hi = idx.max(dim=0).values.cpu().numpy().astype(np.int64)
-        window = (C.c_int32 * 6)(*[int(v) for v in lo], *[int(v) for v in (hi - lo + 2)])
+        idx = volume._index[:nb, :3].to(torch.int64)
+        lo_t = idx.min(dim=0).values
+        n_t = idx.max(dim=0).values - lo_t + 2
+        lo, n = lo_t.cpu().numpy(), n_t.cpu().numpy()
+        window = (C.c_int32 * 6)(*[int(v) for v in lo], *[int(v) for v in n])
+        # bricks in ascending lattice index, not in pool order: triangles come out brick after brick in this order, so the
+        # mesh does not depend on the order the pool handed out its slots in
+        rel = idx - lo_t
+        bricks = torch.sort((rel[:, 0] * n_t[1] + rel[:, 1]) * n_t[2] + rel[:, 2]).indices.to(torch.int32)
         counts = torch.zeros(nb, dtype=torch.int32, device=dev)
         _lib.check(L.gsb_mesh_count(volume._h, window, ptr(bricks), nb, ptr(counts), stream))
         offsets = torch.cumsum(counts.to(torch.int64), 0) - counts.to(torch.int64)
@@ -238,7 +244,7 @@ def extract_triangle_mesh(volume, with_colors: Optional[bool] = None) -> Triangl
         tris = inverse.reshape(-1, 3)
         mesh = TriangleMesh(xyz.cpu().numpy(), tris.cpu().numpy(), None if rgb is None else rgb.cpu().numpy(), device=dev)
         mesh.edge_keys = uniq.cpu().numpy()  # (voxel index inside `key_window` * 3 + axis) per vertex, for tests
-        mesh.key_window = (tuple(int(v) for v in lo), tuple(int(v) for v in (hi - lo + 2)))  # (brick origin, brick count)
+        mesh.key_window = (tuple(int(v) for v in lo), tuple(int(v) for v in n))  # (brick origin, brick count)
     return mesh
 
 

@@ -315,7 +315,10 @@ void gsb_comm_destroy(void* nccl_comm);
  * sorts/uniques the keys (that is the de-duplication Open3D does with a hash map) and asks for the attributes of the
  * unique edges.  The keys must fit 63 bits: 16^3 * nbx * nby * nbz * 3 < 9e18, otherwise GSB_ERR_INVALID.
  *   gsb_mesh_count    tri_counts[b]  = triangles produced by brick b
- *   gsb_mesh_emit     edge_keys[3*t..3*t+2] for every triangle, brick b writing from tri_offsets[b]
+ *   gsb_mesh_emit     edge_keys[3*t..3*t+2] for every triangle, brick b writing from tri_offsets[b]; inside a brick
+ *                     cubes in pool-layout order x*256 + y*16 + z, each cube's triangles in the case table's order,
+ *                     with Open3D's (e0, e2, e1) winding.  Listing the bricks in ascending lattice index gives Open3D's
+ *                     ExtractTriangleMesh loop with its volume units in lattice order, whatever the pool order.
  *   gsb_mesh_vertices xyz and rgb in [0,1] (or NULL) of n unique keys, fp64 [n,3] each, equal to Open3D's doubles
  *                     (one rounding per operation in Open3D's order)
  *   gsb_mesh_vertex_normals TriangleMesh::ComputeVertexNormals() (fp64 [n_vertices,3]) of an indexed mesh, deterministic.

@@ -320,8 +320,10 @@ def _mc_tables():
 def extract_mesh_from_bricks(tw, brick_origin, brick_count, voxel_length, color=None):
     """CPU restatement of ScalableTSDFVolume::ExtractTriangleMesh on a dense brick window
     (tw: [n_bricks,4096,2] as returned by OracleTSDFVolume.export_bricks; unallocated units have weight 0,
-    which is what Open3D's hash-map miss yields).  Returns dict(keys, vertices, colors, triangles):
-    `keys[i]` = (gx,gy,gz,axis) of vertex i in window voxel coordinates, vertices fp64 like Open3D."""
+    which is what Open3D's hash-map miss yields).  Returns dict(keys, vertices, colors, triangles, cubes):
+    `keys[i]` = (gx,gy,gz,axis) of vertex i in window voxel coordinates, vertices fp64 like Open3D, `cubes[t]` = (x,y,z)
+    of the cube triangle t came from, in window voxel coordinates.  Triangles follow the walk over the whole window in
+    x, y, z order, each cube's in the case table's order."""
     shift, edge_shift, e2v, tri = _mc_tables()
     nbx, nby, nbz = (int(v) for v in brick_count)
     g = np.asarray(tw).reshape(nbx, nby, nbz, 16, 16, 16, 2).transpose(0, 3, 1, 4, 2, 5, 6).reshape(nbx * 16, nby * 16, nbz * 16, 2)
@@ -340,7 +342,7 @@ def extract_mesh_from_bricks(tw, brick_origin, brick_count, voxel_length, color=
         valid &= wp[sx:sx + X, sy:sy + Y, sz:sz + Z] != 0
         case |= (fp[sx:sx + X, sy:sy + Y, sz:sz + Z] < 0).astype(np.int32) << i
     active = np.argwhere(valid & (case != 0) & (case != 255))
-    vmap, verts, cols, tris, keys = {}, [], [], [], []
+    vmap, verts, cols, tris, keys, cubes = {}, [], [], [], [], []
     half = voxel_length * 0.5
     b0 = np.asarray(brick_origin, dtype=np.int64) * 16
     for x, y, z in active:
@@ -369,9 +371,10 @@ def extract_mesh_from_bricks(tw, brick_origin, brick_count, voxel_length, color=
             if row[t] < 0:
                 break
             tris.append((idx[int(row[t])], idx[int(row[t + 2])], idx[int(row[t + 1])]))
+            cubes.append((x, y, z))
     return dict(keys=np.array(keys, np.int64).reshape(-1, 4), vertices=np.array(verts, np.float64).reshape(-1, 3),
                 colors=np.array(cols, np.float64).reshape(-1, 3) if col is not None else None,
-                triangles=np.array(tris, np.int64).reshape(-1, 3))
+                triangles=np.array(tris, np.int64).reshape(-1, 3), cubes=np.array(cubes, np.int64).reshape(-1, 3))
 
 
 # ---------------------------------------------------------------------------------------------------------------

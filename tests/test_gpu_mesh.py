@@ -6,6 +6,7 @@ import numpy as np
 import pytest
 
 from tests.test_gpu_tsdf import B0, CX, CY, FX, FY, H, NB, TRUNC, VL, W, _gpu_volume, _views
+from tests.test_oracle_mesh import canonical_triangle_order
 
 pytestmark = pytest.mark.gpu
 
@@ -25,20 +26,11 @@ def _rekey(mesh, b0, nb):
     return ((gx * (nb[1] * 16) + gy) * (nb[2] * 16) + gz) * 3 + axis
 
 
-def _canon(tris):
-    """triangles as a set of rotation-canonical key triples"""
-    out = set()
-    for a, b, c in tris:
-        t = (a, b, c)
-        k = t.index(min(t))
-        out.add((t[k], t[(k + 1) % 3], t[(k + 2) % 3]))
-    return out
-
-
 def test_mesh_matches_open3d_restatement(oracle, gsb_lib, cuda_device):
     import torch
 
     from gs2mesh_b200.mesh import extract_triangle_mesh
+    from tests.test_gpu_mesh_volumes import open3d_vertex_normals
 
     gvol = _gpu_volume(cuda_device, with_color=True)
     for depth, rgb, w2c in _views(5):
@@ -60,11 +52,14 @@ def test_mesh_matches_open3d_restatement(oracle, gsb_lib, cuda_device):
     np.testing.assert_allclose(mesh.vertex_colors, ref["colors"][order], atol=2e-6)
     rank = np.empty(len(order), np.int64)
     rank[order] = np.arange(len(order))
-    assert _canon(map(tuple, mesh.triangles)) == _canon(map(tuple, rank[ref["triangles"]]))
+    want = rank[ref["triangles"][canonical_triangle_order(ref["cubes"])]]
+    np.testing.assert_array_equal(mesh.triangles, want)  # the same triangles, windings and order
 
-    # vertex normals: area-weighted, unit length, pointing away from the object centre
+    # vertex normals: the float64 restatement on the oracle's vertices and triangles; area-weighted, unit length, pointing
+    # away from the object centre
     mesh.compute_vertex_normals(cuda_device)
     n = mesh.vertex_normals
+    np.testing.assert_array_equal(n, open3d_vertex_normals(ref["vertices"][order], want))
     np.testing.assert_allclose(np.linalg.norm(n, axis=1), 1.0, atol=1e-9)
     v, t = mesh.vertices, mesh.triangles
     fn = np.cross(v[t[:, 1]] - v[t[:, 0]], v[t[:, 2]] - v[t[:, 0]])

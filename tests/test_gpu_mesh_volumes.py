@@ -4,11 +4,13 @@
 The volumes are written brick by brick, so they reach what a fused sphere never does: every cube case, every seam between a
 brick and its +1 neighbours, missing neighbours, weight-0 halo voxels, tsdf values of exactly 0, -0 and +-1, subnormals,
 lattice indices far from the origin and at the ends of the 21-bit brick key, and voxel lengths that are not dyadic.  Bars:
-edge keys, vertices, colours and normals bit for bit; triangles as sets."""
+edge keys, vertices, colours and normals bit for bit; triangles as arrays, in the canonical order (bricks in ascending
+lattice index, cubes in pool-layout order inside a brick, the case table's order inside a cube)."""
 import numpy as np
 import pytest
 
-from tests.test_gpu_mesh import _canon, _rekey
+from tests.test_gpu_mesh import _rekey
+from tests.test_oracle_mesh import canonical_triangle_order
 
 pytestmark = pytest.mark.gpu
 
@@ -111,9 +113,12 @@ def _compare(oracle, mesh, units, vl, with_color, b0=None, nb=None):
     loc[sel] = np.arange(int(sel.sum()))
     t = loc[mesh.triangles]
     t = t[(t >= 0).all(1)]
-    assert len(t) == len(ref["triangles"])
-    want = _canon(map(tuple, rank[ref["triangles"]]))
-    assert len(want) == len(ref["triangles"]) and _canon(map(tuple, t)) == want
+    want = rank[ref["triangles"][canonical_triangle_order(ref["cubes"])]]
+    np.testing.assert_array_equal(t, want)  # the same triangles, windings and order
+    # normals: the float64 restatement on the oracle's vertices and triangles, not on the mesh's own arrays
+    if mesh.vertex_normals is None:
+        mesh.compute_vertex_normals(mesh.device)
+    np.testing.assert_array_equal(mesh.vertex_normals[sel], open3d_vertex_normals(ref["vertices"][order], want))
     return len(t)
 
 

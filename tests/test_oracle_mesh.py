@@ -5,6 +5,36 @@ VL = 1.0 / 16
 B0, NB = (-2, -2, -2), (4, 4, 4)
 
 
+def canonical_triangle_order(cubes):
+    """Stable permutation that puts the oracle's triangles (given each one's cube, `cubes` of extract_mesh_from_bricks) in
+    the extracted mesh's order: bricks in ascending lattice index (bx, by, bz), inside a brick cubes in pool-layout order
+    x*256 + y*16 + z, inside a cube the case table's order (the oracle's own, kept by the stable sort)."""
+    c = np.asarray(cubes, np.int64).reshape(-1, 3)
+    b, v = c >> 4, c & 15
+    return np.lexsort((v[:, 2], v[:, 1], v[:, 0], b[:, 2], b[:, 1], b[:, 0]))
+
+
+def test_canonical_order_of_two_bricks(oracle):
+    """Bricks (0,0,0) and (0,1,0): inside voxels at (2,2,2) and (3,3,3) in the first (cube (2,2,2) has both, as opposite
+    corners: two triangles), one at (1,18,1) in the second.  The oracle's x, y, z walk interleaves the bricks; the canonical
+    order finishes the first brick before the second."""
+    t = np.full((16, 32, 16), 0.5, np.float32)  # window voxels [x, y, z]
+    for p in ((2, 2, 2), (3, 3, 3), (1, 18, 1)):
+        t[p] = -0.5
+    tw = np.stack([t.reshape(1, 16, 2, 16, 1, 16).transpose(0, 2, 4, 1, 3, 5).reshape(2, 4096), np.ones((2, 4096), np.float32)],
+                  -1)
+    m = oracle.extract_mesh_from_bricks(tw, (0, 0, 0), (1, 2, 1), VL)
+    first = [(1, 1, 1), (1, 1, 2), (1, 2, 1), (1, 2, 2), (2, 1, 1), (2, 1, 2), (2, 2, 1), (2, 2, 2), (2, 2, 2), (2, 2, 3),
+             (2, 3, 2), (2, 3, 3), (3, 2, 2), (3, 2, 3), (3, 3, 2), (3, 3, 3)]
+    second = [(0, 17, 0), (0, 17, 1), (0, 18, 0), (0, 18, 1), (1, 17, 0), (1, 17, 1), (1, 18, 0), (1, 18, 1)]
+    walk = sorted(first + second)  # the oracle's order: x, y, z over the window
+    assert m["cubes"].tolist() == [list(c) for c in walk]
+    perm = canonical_triangle_order(m["cubes"])
+    assert m["cubes"][perm].tolist() == [list(c) for c in first + second]
+    two = [i for i in perm if tuple(m["cubes"][i]) == (2, 2, 2)]
+    assert len(two) == 2 and two[0] < two[1]  # the case table's order inside the cube
+
+
 def _sphere_bricks(radius=0.55, trunc=0.2, hole=False):
     n = 64
     c = (np.arange(n) + 0.5) * VL + B0[0] * 16 * VL
