@@ -6,12 +6,13 @@ Marching cubes, vertex attributes and vertex normals run on the GPU (gsb_mesh_* 
 include/gs2mesh_b200.h); vertex de-duplication is a sort/unique of 64-bit edge keys (what Open3D
 does with a hash map).  Connected-component cleaning runs on the GPU for a mesh extracted from a
 GPU volume (`TriangleMesh.device` is set) and with numpy / scipy for a mesh built from host arrays;
-both give the same labels, counts and cleaned mesh.  PLY writing stays on the host like in the
-reference.
+both give the same labels, counts and cleaned mesh.  Vertex-clustering simplification (Open3D's
+simplify_vertex_clustering) runs on the GPU.  PLY writing stays on the host like in the reference.
 """
 from __future__ import annotations
 
 import ctypes as C
+import enum
 from typing import Optional
 
 import numpy as np
@@ -30,6 +31,13 @@ def color_to_uint8(colors):
     s = np.where(c < 1.0, c, 1.0) * 255.0
     lo = np.floor(s)
     return (lo + (s - lo >= 0.5)).astype(np.uint8)
+
+
+class SimplificationContraction(enum.IntEnum):
+    """open3d.geometry.SimplificationContraction: where simplify_vertex_clustering places a cell's vertex."""
+
+    Average = 0  # GSB_SIMPLIFY_AVERAGE: the mean of the cell's vertices
+    Quadric = 1  # GSB_SIMPLIFY_QUADRIC: the minimum of the cell's plane quadrics
 
 
 class TriangleMesh:
@@ -155,6 +163,54 @@ class TriangleMesh:
             tris, used = out_tri[:kt].cpu().numpy(), ids[:kv].cpu().numpy()
         pick = lambda a: None if a is None else a[used]
         return TriangleMesh(self.vertices[used], tris, pick(self.vertex_colors), pick(self.vertex_normals), device=self.device)
+
+    # -- TriangleMesh::SimplifyVertexClustering (DESIGN.md section 7, "Simplification")
+    def simplify_vertex_clustering(self, voxel_size, contraction=None):
+        """A new mesh of the same class with one vertex per occupied cell of a `voxel_size` grid anchored half a cell
+        below the vertices' minimum.  Cells are numbered in the order of their smallest vertex id (Open3D's numbering).
+        SimplificationContraction.Average (the default) places each at the mean of its vertices, Quadric at the
+        minimum of its triangles' area-weighted plane quadrics where |det A| > 1e-4 (the mean elsewhere); colours and
+        normals are means either way.  Triangles whose corners fall into fewer than three cells are dropped, the rest
+        start at their smallest vertex id (winding kept) and each such triple is kept once, in input order.
+
+        Runs on `self.device` (the current CUDA device for a mesh built from host arrays); the result records that
+        device and holds host arrays.  `self.last_simplify_stats` gives the cells, the triangles and the cells that
+        took the quadric solve.  RuntimeError("voxel_size <= 0.0") / ("voxel_size is too small.") as in Open3D;
+        ValueError for non-finite vertices or voxel size, bad indices or a cell box past 63-bit keys."""
+        contraction = SimplificationContraction.Average if contraction is None else SimplificationContraction(contraction)
+        s = float(voxel_size)
+        if not s > 0.0:
+            raise RuntimeError("voxel_size <= 0.0")
+        nv, nt = len(self.vertices), len(self.triangles)
+        if nt and (self.triangles.min() < 0 or self.triangles.max() >= nv):
+            raise ValueError("simplify_vertex_clustering: triangle vertex index out of range")
+        for name in ("vertex_colors", "vertex_normals"):
+            a = getattr(self, name)
+            if a is not None and len(a) != nv:
+                raise ValueError(f"simplify_vertex_clustering: {name} must have one row per vertex")
+        lo = self.vertices.min(axis=0) if nv else np.zeros(3)
+        hi = self.vertices.max(axis=0) if nv else np.zeros(3)
+        dev = _lib.device(self.device)
+        L = _lib.lib()
+        dbl3 = C.c_double * 3
+        with torch.cuda.device(dev):
+            up = lambda a: None if a is None else torch.as_tensor(a).to(dev).contiguous()
+            xyz, rgb, nrm, tri = up(self.vertices), up(self.vertex_colors), up(self.vertex_normals), up(self.triangles)
+            like = lambda a: None if a is None else torch.empty_like(a)
+            out_v, out_c, out_n, out_t = like(xyz), like(rgb), like(nrm), like(tri)
+            work = torch.empty(L.gsb_mesh_simplify_workspace_bytes(nv, nt), dtype=torch.uint8, device=dev)
+            sizes = torch.empty(3, dtype=torch.int64, device=dev)
+            rc = L.gsb_mesh_simplify(ptr(xyz), ptr(rgb), ptr(nrm), nv, ptr(tri), nt, dbl3(*lo.tolist()), dbl3(*hi.tolist()), s,
+                                     int(contraction), ptr(work), work.numel(), ptr(out_v), ptr(out_c), ptr(out_n), ptr(out_t),
+                                     ptr(sizes), _lib.stream(dev))
+            if rc == _lib.GSB_ERR_INVALID and L.gsb_last_error().endswith(b"voxel_size is too small."):
+                raise RuntimeError("voxel_size is too small.")
+            _lib.check(rc, invalid_is_value_error=True)
+            k, kt, kq = (int(x) for x in sizes.cpu().tolist())
+            host = lambda a, n: None if a is None else a[:n].cpu().numpy()
+            out = type(self)(host(out_v, k), host(out_t, kt), host(out_c, k), host(out_n, k), device=dev)
+        self.last_simplify_stats = {"vertices": k, "triangles": kt, "quadric_cells": kq}
+        return out
 
     # -- o3d.io.write_triangle_mesh(path, mesh): binary little-endian PLY, double coordinates
     def write_ply(self, path):

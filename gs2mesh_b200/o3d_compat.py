@@ -19,6 +19,10 @@ and Open3D's other two read-outs of the volume, which the evaluators take as inp
     vox = volume.extract_voxel_point_cloud()    # voxel centres near the surface, grey by tsdf
     o3d.io.write_point_cloud(path, pcd)
 
+and the simplification users run on the cleaned mesh:
+
+    small = mesh.simplify_vertex_clustering(voxel_size, o3d.geometry.SimplificationContraction.Average)
+
 Differences from Open3D, by construction: the volume lives in GPU memory (an unbounded, hashed set of 16^3 bricks on
 the same voxel lattice, like Open3D's; `window_resolution=` only sets the window dense read-backs look at); images are uploaded on
 integrate().  Everything else (argument names, the RuntimeError on mismatching image sizes, float32 depth
@@ -32,6 +36,7 @@ from types import SimpleNamespace
 import numpy as np
 
 from .mesh import PointCloud as _PointCloud
+from .mesh import SimplificationContraction
 from .mesh import TriangleMesh as _Mesh
 from .mesh import extract_point_cloud as _extract_pcd
 from .mesh import extract_triangle_mesh as _extract
@@ -180,7 +185,8 @@ def _verbosity(_level):
 
 
 # module tree mirroring `open3d`
-geometry = SimpleNamespace(Image=Image, RGBDImage=RGBDImage, TriangleMesh=TriangleMesh, PointCloud=PointCloud)
+geometry = SimpleNamespace(Image=Image, RGBDImage=RGBDImage, TriangleMesh=TriangleMesh, PointCloud=PointCloud,
+                           SimplificationContraction=SimplificationContraction)
 camera = SimpleNamespace(PinholeCameraIntrinsic=PinholeCameraIntrinsic)
 pipelines = SimpleNamespace(integration=SimpleNamespace(ScalableTSDFVolume=ScalableTSDFVolume, TSDFVolumeColorType=TSDFVolumeColorType))
 io = SimpleNamespace(write_triangle_mesh=_write_triangle_mesh, write_point_cloud=_write_point_cloud)

@@ -358,6 +358,32 @@ int gsb_mesh_remove_small_clusters(const int64_t* triangles, int64_t n_triangles
                                    const int64_t* counts, double threshold, void* workspace, size_t workspace_bytes,
                                    int64_t* out_triangles, int64_t* vertex_ids, int64_t* sizes, void* stream);
 
+/* Vertex-clustering simplification: TriangleMesh::SimplifyVertexClustering(voxel_size, contraction) of Open3D 0.17.0
+ * (DESIGN.md section 7, "Simplification"; restated in tests/simplify_oracle.py).  vertices: device double [n_vertices,3];
+ * colors / normals: device double [n_vertices,3] or NULL; triangles: device int64 [n_triangles,3], every index in
+ * [0, n_vertices) (not checked on the device); n_vertices and n_triangles <= 2^31 - 1.  min_bound / max_bound: host
+ * double[3], the component-wise min and max of the vertices (any finite values when n_vertices is 0).  With s =
+ * voxel_size and m = min_bound - s*0.5, vertex v lies in cell floor((v - m) / s) (one rounded subtraction, one rounded
+ * division).  GSB_ERR_INVALID when s <= 0 or NaN ("voxel_size <= 0.0") or infinite, the bounds are not finite, s * INT_MAX
+ * < max_k((max_bound_k + s*0.5) - m_k) ("voxel_size is too small."), or the cell box holds more than 2^63 cells.
+ *   Each occupied cell is one output vertex, numbered in the order of its smallest vertex id.  Its position, colour and
+ *   normal are the sums over its vertices in ascending id, from 0.0, divided by double(count) (normals not
+ *   renormalised).  GSB_SIMPLIFY_QUADRIC instead adds, for each vertex of the cell in ascending id and each distinct
+ *   triangle incident to it in ascending id, the triangle's plane quadric weighted by its area, and takes -A^-1 b
+ *   (Eigen's pivoted LDLT) when |det A| > 1e-4; colours and normals are still averaged.
+ *   Triangles are mapped to cells, dropped when two corners share a cell, rotated so the smallest id comes first
+ *   (winding kept), and the first occurrence of each rotated triple is kept, in input order.
+ * out_vertices / out_colors / out_normals: device double [n_vertices,3] (colours and normals only when given);
+ * out_triangles: device int64 [n_triangles,3]; sizes: device int64[3] = (vertices, triangles, cells that took the
+ * quadric solve).  One caller workspace of gsb_mesh_simplify_workspace_bytes() (0 for invalid sizes); no host sync. */
+#define GSB_SIMPLIFY_AVERAGE 0
+#define GSB_SIMPLIFY_QUADRIC 1
+size_t gsb_mesh_simplify_workspace_bytes(int64_t n_vertices, int64_t n_triangles);
+int gsb_mesh_simplify(const double* vertices, const double* colors, const double* normals, int64_t n_vertices,
+                      const int64_t* triangles, int64_t n_triangles, const double* min_bound, const double* max_bound,
+                      double voxel_size, int contraction, void* workspace, size_t workspace_bytes, double* out_vertices,
+                      double* out_colors, double* out_normals, int64_t* out_triangles, int64_t* sizes, void* stream);
+
 /* ------------------------------------------------------------------------------------------
  * Point clouds: volume.extract_point_cloud() / extract_voxel_point_cloud()
  * (Open3D ScalableTSDFVolume::ExtractPointCloud / ExtractVoxelPointCloud; DESIGN.md section 7, "Point clouds")
