@@ -158,8 +158,10 @@ __global__ void __launch_bounds__(256) visibility_kernel(const double* __restric
     const double u = __ddiv_rn(__dsub_rn(v[3 * i + a], mins[a]), vs);
     const double gd = __dsub_rn(__dmul_rn(__ddiv_rn(u, (double)(res[a] - 1)), 2.0), 1.0);
     const float g = __double2float_rn(gd);
-    // grid_sampler_compute_source_index (align_corners) then nearbyint and the cast to int (saturating, NaN -> 0)
-    idx[a] = __float2int_rn(__fmul_rn(__fdiv_rn(__fadd_rn(g, 1.0f), 2.0f), (float)(res[a] - 1)));
+    // grid_sampler_compute_source_index (align_corners), whose safe_downgrade_to_int_range sends a non-finite coordinate
+    // outside the volume; then nearbyint and the cast to int (saturating: finite values beyond int fall outside too)
+    const float x = __fmul_rn(__fdiv_rn(__fadd_rn(g, 1.0f), 2.0f), (float)(res[a] - 1));
+    idx[a] = isfinite(x) ? __float2int_rn(x) : -1;
     inside = inside && idx[a] >= 0 && idx[a] < res[a];
   }
   keep[i] = inside && volume[((long long)idx[0] * r1 + idx[1]) * r2 + idx[2]] != 0;
@@ -271,9 +273,14 @@ int gsb_eval_poisson_eliminate(const int64_t* offsets, const int32_t* neighbours
 int gsb_eval_visibility(const double* vertices, int64_t n_vertices, const double* min_pts, double voxel_size,
                         const int32_t* resolution, const uint8_t* volume, uint8_t* keep, void* stream_v) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
+  // a non-finite or non-positive voxel size, or a non-finite min_pts, would map every vertex to voxel 0 or to none
   if (n_vertices < 0 || !min_pts || !resolution || resolution[0] < 2 || resolution[1] < 2 || resolution[2] < 2 ||
-      (double)resolution[0] * resolution[1] * resolution[2] > 9e15 || (n_vertices && (!vertices || !volume || !keep)))
-    return fail(GSB_ERR_INVALID, "eval_visibility: bad arguments (every resolution must be >= 2)");
+      (double)resolution[0] * resolution[1] * resolution[2] > 9e15 || !(voxel_size > 0.0) || !(voxel_size < INFINITY) ||
+      !isfinite(min_pts[0]) || !isfinite(min_pts[1]) || !isfinite(min_pts[2]) ||
+      (n_vertices && (!vertices || !volume || !keep)))
+    return fail(GSB_ERR_INVALID,
+                "eval_visibility: bad arguments (every resolution must be >= 2, voxel_size finite and > 0, min_pts "
+                "finite)");
   if (n_vertices == 0) return GSB_OK;
   visibility_kernel<<<(unsigned)((n_vertices + 255) / 256), 256, 0, stream>>>(vertices, n_vertices, min_pts[0], min_pts[1],
                                                                               min_pts[2], voxel_size, resolution[0],

@@ -169,7 +169,8 @@ def sample_points_poisson_disk(vertices, triangles, number_of_points, init_facto
 
 def visibility_test(vertices, volume, min_pts, resolution, voxel_size, device=None):
     """evaluate.py:34-41's visibility: device bool [N], True where the nearest voxel of `volume` (reshaped to
-    `resolution`, read as D, H, W) is > 0 as a float32, False outside the volume."""
+    `resolution`, read as D, H, W) is > 0 as a float32, False outside the volume.  Raises ValueError for a resolution
+    below 2 on any axis, a voxel_size that is not finite and > 0, or a min_pts that is not finite."""
     v = _points(vertices, _lib.device(device, vertices))
     dev = v.device
     res = np.asarray(resolution).astype(np.int64).reshape(3)

@@ -584,8 +584,10 @@ int gsb_eval_cull_vertices_by_masks(const double* vertices, int64_t n_vertices, 
  *   gsb_eval_visibility         keep[i] = 1 iff grid_sample(volume, g, nearest, zeros, align_corners=True) > 0 for
  *                               g = fp32(((((p - min_pts)/voxel_size) / (res - 1)) * 2) - 1) (fp64 until the rounding), axes
  *                               reordered to (z, y, x); volume: device uint8 [res0][res1][res2], nonzero where the
- *                               reference's float volume is > 0.  min_pts: host double [3]; resolution: host int32 [3], each
- *                               >= 2. */
+ *                               reference's float volume is > 0; a vertex whose source coordinate is NaN or infinite is
+ *                               outside, as in torch's sampler.  min_pts: host double [3], finite; voxel_size: finite and
+ *                               > 0; resolution: host int32 [3], each >= 2, their product at most 9e15.  The voxel index
+ *                               is computed in 64 bits, so volumes of more than 2^31 voxels work. */
 int gsb_eval_triangle_areas(const double* vertices, int64_t n_vertices, const int64_t* triangles, int64_t n_triangles,
                             double* areas, void* stream);
 int gsb_eval_sample_uniform(const double* vertices, int64_t n_vertices, const int64_t* triangles, int64_t n_triangles,

@@ -246,11 +246,13 @@ def visibility_index(points, min_pts, resolution, voxel_size):
     v = (p - np.asarray(min_pts, np.float64).reshape(3)) / np.float64(voxel_size)
     g = (v / (res - 1) * 2 - 1).astype(np.float32)
     idx = np.empty((len(p), 3), np.int64)
-    with np.errstate(invalid="ignore"):
+    with np.errstate(invalid="ignore", over="ignore"):
         for a in range(3):
             x = ((g[:, a] + np.float32(1)) / np.float32(2)) * np.float32(res[a] - 1)
-            r = np.rint(x).astype(np.float64)  # nearbyint in fp32, then the saturating conversion (NaN -> 0)
-            idx[:, a] = np.where(np.isnan(r), 0, np.clip(r, -2 ** 31, 2 ** 31 - 1)).astype(np.int64)
+            # grid_sampler's safe_downgrade_to_int_range: a non-finite coordinate becomes -100, outside the volume;
+            # otherwise nearbyint in fp32, then the saturating conversion
+            r = np.where(np.isfinite(x), np.rint(x), -100.0).astype(np.float64)
+            idx[:, a] = np.clip(r, -2 ** 31, 2 ** 31 - 1).astype(np.int64)
     return idx
 
 
