@@ -14,6 +14,7 @@ LIB_PATH = os.path.join(_PKG, "libgs2mesh_b200.so")
 GSB_OK, GSB_ERR_INVALID, GSB_ERR_WORKSPACE, GSB_ERR_CUDA, GSB_ERR_ALIGNMENT = range(5)
 GSB_PCD_SURFACE, GSB_PCD_VOXELS = 0, 1  # gsb_pcd_* mode
 GSB_SIMPLIFY_AVERAGE, GSB_SIMPLIFY_QUADRIC = 0, 1  # gsb_mesh_simplify contraction
+GSB_FILTER_SIMPLE, GSB_FILTER_LAPLACIAN, GSB_FILTER_TAUBIN, GSB_FILTER_SHARPEN = range(4)  # gsb_mesh_filter kind
 
 RASTER_EXACT_TILE_CULL = 1
 RASTER_NO_TMA = 2
@@ -98,6 +99,9 @@ SIGNATURES = {
     "gsb_mesh_simplify_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int64]),
     "gsb_mesh_simplify": (C.c_int, [_vp, _vp, _vp, C.c_int64, _vp, C.c_int64, C.POINTER(C.c_double), C.POINTER(C.c_double),
                                     C.c_double, C.c_int, _vp, C.c_size_t, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "gsb_mesh_filter_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int, C.c_int]),
+    "gsb_mesh_filter": (C.c_int, [C.c_int, _vp, _vp, _vp, C.c_int64, _vp, _vp, C.c_int32, C.c_double, C.c_double, C.c_int,
+                                  _vp, C.c_size_t, _vp, _vp, _vp, _vp]),
     "gsb_pcd_count":(C.c_int, [_vp, C.POINTER(C.c_int32), _vp, C.c_uint32, C.c_int, _vp, _vp]),
     "gsb_pcd_emit": (C.c_int, [_vp, C.POINTER(C.c_int32), _vp, C.c_uint32, C.c_int, _vp, _vp, _vp]),
     "gsb_pcd_points": (C.c_int, [_vp, C.POINTER(C.c_int32), _vp, C.c_int64, C.c_int, _vp, _vp, _vp, _vp]),

@@ -7,7 +7,8 @@ include/gs2mesh_b200.h); vertex de-duplication is a sort/unique of 64-bit edge k
 does with a hash map).  Connected-component cleaning runs on the GPU for a mesh extracted from a
 GPU volume (`TriangleMesh.device` is set) and with numpy / scipy for a mesh built from host arrays;
 both give the same labels, counts and cleaned mesh.  Vertex-clustering simplification (Open3D's
-simplify_vertex_clustering) runs on the GPU.  PLY writing stays on the host like in the reference.
+simplify_vertex_clustering) and the smoothing and sharpening filters (filter_smooth_simple / _laplacian / _taubin,
+filter_sharpen) run on the GPU.  PLY writing stays on the host like in the reference.
 """
 from __future__ import annotations
 
@@ -38,6 +39,27 @@ class SimplificationContraction(enum.IntEnum):
 
     Average = 0  # GSB_SIMPLIFY_AVERAGE: the mean of the cell's vertices
     Quadric = 1  # GSB_SIMPLIFY_QUADRIC: the minimum of the cell's plane quadrics
+
+
+class FilterScope(enum.IntEnum):
+    """open3d.geometry.FilterScope: which vertex attributes the smoothing and sharpening filters change."""
+
+    All = 0  # GSB_FILTER_SCOPE_ALL: positions, and colours and normals where the mesh has them
+    Color = 1
+    Normal = 2
+    Vertex = 3  # positions only
+
+
+def _adjacency(tri, nv):
+    """Open3D's ComputeAdjacencyList as CSR on tri's device: (offsets int64 [nv + 1], neighbours int64), each vertex's
+    run holding the distinct ids it shares a triangle with at another corner position, ascending."""
+    src = tri[:, [0, 0, 1, 1, 2, 2]].reshape(-1)
+    dst = tri[:, [1, 2, 0, 2, 0, 1]].reshape(-1)
+    keys = torch.unique(src * nv + dst)  # sorted: by vertex, then by neighbour
+    owner = keys // nv
+    offsets = torch.zeros(nv + 1, dtype=torch.int64, device=tri.device)
+    offsets[1:] = torch.cumsum(torch.bincount(owner, minlength=nv), 0)
+    return offsets, (keys - owner * nv).contiguous()
 
 
 class TriangleMesh:
@@ -211,6 +233,60 @@ class TriangleMesh:
             out = type(self)(host(out_v, k), host(out_t, kt), host(out_c, k), host(out_n, k), device=dev)
         self.last_simplify_stats = {"vertices": k, "triangles": kt, "quadric_cells": kq}
         return out
+
+    # -- TriangleMesh::FilterSmoothSimple / FilterSmoothLaplacian / FilterSmoothTaubin / FilterSharpen (DESIGN.md
+    # section 7, "Smoothing and sharpening").  Each returns a new mesh of the same class with the same triangles; it runs
+    # on `self.device` (the current CUDA device for a mesh built from host arrays), and the result records that device
+    # and holds host arrays.  Neighbours are the vertices sharing a triangle; each pass reads only the previous pass's
+    # values.  `filter_scope` picks positions (Vertex), colours (Color), normals (Normal) or all three (All); colours and
+    # normals only where the mesh has them, normals not renormalised, colours not clamped.
+    def filter_smooth_simple(self, number_of_iterations=1, filter_scope=FilterScope.All):
+        """x' = (x + sum of the neighbours' x) / (1 + number of neighbours), per pass."""
+        return self._filter("filter_smooth_simple", _lib.GSB_FILTER_SIMPLE, number_of_iterations, 0.0, 0.0, filter_scope)
+
+    def filter_smooth_laplacian(self, number_of_iterations=1, lambda_filter=0.5, filter_scope=FilterScope.All):
+        """x' = x + lambda_filter * (the neighbours' x weighted by 1 / (distance + 1e-12), averaged, - x), per pass; a
+        vertex without neighbours keeps its values."""
+        return self._filter("filter_smooth_laplacian", _lib.GSB_FILTER_LAPLACIAN, number_of_iterations, lambda_filter, 0.0,
+                            filter_scope)
+
+    def filter_smooth_taubin(self, number_of_iterations=1, lambda_filter=0.5, mu=-0.53, filter_scope=FilterScope.All):
+        """Per iteration one Laplacian pass with lambda_filter, then one with mu: smooths without shrinking."""
+        return self._filter("filter_smooth_taubin", _lib.GSB_FILTER_TAUBIN, number_of_iterations, lambda_filter, mu,
+                            filter_scope)
+
+    def filter_sharpen(self, number_of_iterations=1, strength=1, filter_scope=FilterScope.All):
+        """x' = x + strength * sum over the neighbours of (x - neighbour's x), per pass."""
+        return self._filter("filter_sharpen", _lib.GSB_FILTER_SHARPEN, number_of_iterations, strength, 0.0, filter_scope)
+
+    def _filter(self, name, kind, number_of_iterations, param0, param1, filter_scope):
+        """gsb_mesh_filter on the mesh's CSR adjacency: the one call path of the four filters."""
+        scope = FilterScope(filter_scope)
+        iterations = int(number_of_iterations)
+        if not 0 <= iterations <= 2**31 - 1:
+            raise ValueError(f"{name}: number_of_iterations must be in [0, 2^31 - 1], got {iterations}")
+        nv, nt = len(self.vertices), len(self.triangles)
+        if nt and (self.triangles.min() < 0 or self.triangles.max() >= nv):
+            raise ValueError(f"{name}: triangle vertex index out of range")
+        for attr in ("vertex_colors", "vertex_normals"):
+            a = getattr(self, attr)
+            if a is not None and len(a) != nv:
+                raise ValueError(f"{name}: {attr} must have one row per vertex")
+        dev = _lib.device(self.device)
+        L = _lib.lib()
+        with torch.cuda.device(dev):
+            up = lambda a: None if a is None else torch.as_tensor(a).to(dev).contiguous()
+            xyz, rgb, nrm = up(self.vertices), up(self.vertex_colors), up(self.vertex_normals)
+            offsets, neighbours = _adjacency(up(self.triangles), nv)
+            like = lambda a: None if a is None else torch.empty_like(a)
+            out_v, out_c, out_n = like(xyz), like(rgb), like(nrm)
+            work = torch.empty(L.gsb_mesh_filter_workspace_bytes(nv, rgb is not None, nrm is not None), dtype=torch.uint8,
+                               device=dev)
+            _lib.check(L.gsb_mesh_filter(kind, ptr(xyz), ptr(rgb), ptr(nrm), nv, ptr(offsets), ptr(neighbours), iterations,
+                                         float(param0), float(param1), int(scope), ptr(work), work.numel(), ptr(out_v),
+                                         ptr(out_c), ptr(out_n), _lib.stream(dev)), invalid_is_value_error=True)
+            host = lambda a: None if a is None else a.cpu().numpy()
+            return type(self)(host(out_v), self.triangles.copy(), host(out_c), host(out_n), device=dev)
 
     # -- o3d.io.write_triangle_mesh(path, mesh): binary little-endian PLY, double coordinates
     def write_ply(self, path):

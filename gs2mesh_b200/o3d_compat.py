@@ -23,6 +23,11 @@ and the simplification users run on the cleaned mesh:
 
     small = mesh.simplify_vertex_clustering(voxel_size, o3d.geometry.SimplificationContraction.Average)
 
+and the filters that remove the fused mesh's voxel-scale ripple (each returns a new mesh):
+
+    smooth = mesh.filter_smooth_taubin(10)      # also filter_smooth_laplacian, filter_smooth_simple, filter_sharpen
+    smooth = mesh.filter_smooth_laplacian(5, 0.5, o3d.geometry.FilterScope.Vertex)
+
 Differences from Open3D, by construction: the volume lives in GPU memory (an unbounded, hashed set of 16^3 bricks on
 the same voxel lattice, like Open3D's; `window_resolution=` only sets the window dense read-backs look at); images are uploaded on
 integrate().  Everything else (argument names, the RuntimeError on mismatching image sizes, float32 depth
@@ -36,7 +41,7 @@ from types import SimpleNamespace
 import numpy as np
 
 from .mesh import PointCloud as _PointCloud
-from .mesh import SimplificationContraction
+from .mesh import FilterScope, SimplificationContraction
 from .mesh import TriangleMesh as _Mesh
 from .mesh import extract_point_cloud as _extract_pcd
 from .mesh import extract_triangle_mesh as _extract
@@ -186,7 +191,7 @@ def _verbosity(_level):
 
 # module tree mirroring `open3d`
 geometry = SimpleNamespace(Image=Image, RGBDImage=RGBDImage, TriangleMesh=TriangleMesh, PointCloud=PointCloud,
-                           SimplificationContraction=SimplificationContraction)
+                           SimplificationContraction=SimplificationContraction, FilterScope=FilterScope)
 camera = SimpleNamespace(PinholeCameraIntrinsic=PinholeCameraIntrinsic)
 pipelines = SimpleNamespace(integration=SimpleNamespace(ScalableTSDFVolume=ScalableTSDFVolume, TSDFVolumeColorType=TSDFVolumeColorType))
 io = SimpleNamespace(write_triangle_mesh=_write_triangle_mesh, write_point_cloud=_write_point_cloud)

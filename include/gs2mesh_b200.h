@@ -384,6 +384,41 @@ int gsb_mesh_simplify(const double* vertices, const double* colors, const double
                       double voxel_size, int contraction, void* workspace, size_t workspace_bytes, double* out_vertices,
                       double* out_colors, double* out_normals, int64_t* out_triangles, int64_t* sizes, void* stream);
 
+/* Smoothing and sharpening: TriangleMesh::FilterSmoothSimple / FilterSmoothLaplacian / FilterSmoothTaubin /
+ * FilterSharpen of Open3D 0.17.0 (DESIGN.md section 7, "Smoothing and sharpening"; restated in tests/filter_oracle.py).
+ * vertices: device double [n_vertices,3]; colors / normals: device double [n_vertices,3] or NULL; n_vertices <= 2^31 - 1.
+ * The neighbours N(v) come as CSR: adjacency_offsets: device int64 [n_vertices + 1]; neighbours: device int64
+ * [offsets[n_vertices]] (NULL allowed when that is 0), the run [offsets[v], offsets[v+1]) holding the distinct ids u that
+ * share a triangle with v at another corner position (Open3D's ComputeAdjacencyList: a degenerate (a,a,b) makes a its
+ * own neighbour), sorted ascending within the run; neither is checked on the device.
+ *   One pass, every fp64 operation rounded once, sums from 0.0 over N(v) in ascending id, x a filtered attribute, p the
+ *   pass's input positions, deg = |N(v)|:
+ *   GSB_FILTER_SIMPLE     x' = (x + sum x_u) / double(1 + deg)
+ *   GSB_FILTER_LAPLACIAN  w_u = 1.0 / (sqrt((dx*dx + dy*dy) + dz*dz) + 1e-12) with d = p_v - p_u, W = sum w_u;
+ *                         x' = x + param0 * ((sum (w_u * x_u)) / W - x); a vertex with deg = 0 keeps x
+ *   GSB_FILTER_TAUBIN     a Laplacian pass with param0 (lambda), then one with param1 (mu), per iteration
+ *   GSB_FILTER_SHARPEN    x' = x + param0 * sum (x - x_u)
+ * scope (GSB_FILTER_SCOPE_*, Open3D's FilterScope): positions are filtered for ALL and VERTEX, colours for ALL and COLOR,
+ * normals for ALL and NORMAL; an attribute that is not filtered (or every attribute when iterations is 0) is copied.
+ * Normals are not renormalised, colours not clamped.  Each pass reads only the previous pass's values.
+ * out_vertices / out_colors / out_normals: device double [n_vertices,3], given exactly when the matching input is, not
+ * overlapping any input (the inputs are never written).  GSB_ERR_INVALID for an unknown kind or scope, iterations < 0, a
+ * negative n_vertices or one past 32-bit ids, a missing pointer, or an output without its input.  One caller workspace
+ * of gsb_mesh_filter_workspace_bytes() (0 for invalid sizes), else GSB_ERR_WORKSPACE; no host sync. */
+#define GSB_FILTER_SIMPLE 0
+#define GSB_FILTER_LAPLACIAN 1
+#define GSB_FILTER_TAUBIN 2
+#define GSB_FILTER_SHARPEN 3
+#define GSB_FILTER_SCOPE_ALL 0
+#define GSB_FILTER_SCOPE_COLOR 1
+#define GSB_FILTER_SCOPE_NORMAL 2
+#define GSB_FILTER_SCOPE_VERTEX 3
+size_t gsb_mesh_filter_workspace_bytes(int64_t n_vertices, int with_colors, int with_normals);
+int gsb_mesh_filter(int kind, const double* vertices, const double* colors, const double* normals, int64_t n_vertices,
+                    const int64_t* adjacency_offsets, const int64_t* neighbours, int32_t iterations, double param0,
+                    double param1, int scope, void* workspace, size_t workspace_bytes, double* out_vertices, double* out_colors,
+                    double* out_normals, void* stream);
+
 /* ------------------------------------------------------------------------------------------
  * Point clouds: volume.extract_point_cloud() / extract_voxel_point_cloud()
  * (Open3D ScalableTSDFVolume::ExtractPointCloud / ExtractVoxelPointCloud; DESIGN.md section 7, "Point clouds")
