@@ -102,6 +102,15 @@ SIGNATURES = {
     "gsb_mesh_filter_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int, C.c_int]),
     "gsb_mesh_filter": (C.c_int, [C.c_int, _vp, _vp, _vp, C.c_int64, _vp, _vp, C.c_int32, C.c_double, C.c_double, C.c_int,
                                   _vp, C.c_size_t, _vp, _vp, _vp, _vp]),
+    "gsb_mesh_edge_topology_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int64]),
+    "gsb_mesh_edge_topology": (C.c_int, [_vp, C.c_int64, C.c_int64, C.c_int, _vp, C.c_size_t, _vp, _vp, _vp]),
+    "gsb_mesh_vertex_topology_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int64]),
+    "gsb_mesh_non_manifold_vertices": (C.c_int, [_vp, C.c_int64, C.c_int64, _vp, C.c_size_t, _vp, _vp, _vp]),
+    "gsb_mesh_self_intersections_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int64, C.c_int64]),
+    "gsb_mesh_self_intersections": (C.c_int, [_vp, C.c_int64, _vp, C.c_int64, C.POINTER(C.c_double), C.POINTER(C.c_double),
+                                              _vp, C.c_size_t, _vp, C.c_int64, _vp, _vp]),
+    "gsb_mesh_area_volume_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int64]),
+    "gsb_mesh_area_volume": (C.c_int, [_vp, C.c_int64, _vp, C.c_int64, _vp, C.c_size_t, _vp, _vp]),
     "gsb_pcd_count":(C.c_int, [_vp, C.POINTER(C.c_int32), _vp, C.c_uint32, C.c_int, _vp, _vp]),
     "gsb_pcd_emit": (C.c_int, [_vp, C.POINTER(C.c_int32), _vp, C.c_uint32, C.c_int, _vp, _vp, _vp]),
     "gsb_pcd_points": (C.c_int, [_vp, C.POINTER(C.c_int32), _vp, C.c_int64, C.c_int, _vp, _vp, _vp, _vp]),

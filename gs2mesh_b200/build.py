@@ -14,7 +14,7 @@ CSRC = os.path.join(PKG_DIR, "csrc")
 LIB_PATH = os.path.join(PKG_DIR, "libgs2mesh_b200.so")
 SOURCES = ["gsb_raster.cu", "gsb_tsdf.cu", "gsb_mesh.cu", "gsb_reduce.cu", "gsb_eval.cu", "gsb_cull.cu", "gsb_stereo.cu",
            "gsb_tnt.cu", "gsb_mobilebrick.cu", "gsb_normals.cu", "gsb_pointcloud.cu", "gsb_raycast.cu", "gsb_simplify.cu",
-           "gsb_filter.cu"]
+           "gsb_filter.cu", "gsb_topology.cu"]
 NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
               "-Xcompiler", "-fPIC", "-shared", "-I", os.path.join(ROOT, "include"), "-I", CSRC, "-ldl"]
 

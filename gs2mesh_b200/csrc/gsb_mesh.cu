@@ -23,6 +23,7 @@
 #include "gs2mesh_b200.h"
 #include "gsb_common.h"
 #include "gsb_mc_tables.h"
+#include "gsb_union_find.cuh"
 #include "gsb_volume_view.cuh"
 
 
@@ -187,43 +188,9 @@ __global__ void __launch_bounds__(256) mesh_vertex_normals_kernel(const double* 
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
-// Edge-connected triangle clusters.  Union-find over triangle ids in the style of ECL-CC: a larger root is always hooked
-// under a smaller one with atomicCAS, so parent[t] <= t holds at every moment and the surviving root of a cluster is its
-// smallest triangle.  Parents are read with relaxed atomic loads; finds halve the path they walk.  Only roots are ever
-// CAS'd and a non-root never becomes a root again, so a path-halving store (an ancestor into a non-root) cannot undo a
-// hook.
+// Edge-connected triangle clusters: the union-find of gsb_union_find.cuh over triangle ids, so the surviving root of a
+// cluster is its smallest triangle.
 // ---------------------------------------------------------------------------------------------------------------------
-using ParentRef = cuda::atomic_ref<int, cuda::thread_scope_device>;
-
-__device__ __forceinline__ int uf_load(int* parent, int x) { return ParentRef(parent[x]).load(cuda::memory_order_relaxed); }
-
-__device__ __forceinline__ int uf_find(int* parent, int x) {
-  int p = uf_load(parent, x);
-  while (p != x) {
-    const int gp = uf_load(parent, p);
-    if (gp != p) ParentRef(parent[x]).store(gp, cuda::memory_order_relaxed);
-    x = gp;
-    p = uf_load(parent, x);
-  }
-  return x;
-}
-
-__device__ __forceinline__ void uf_union(int* parent, int a, int b) {
-  a = uf_find(parent, a);
-  b = uf_find(parent, b);
-  while (a != b) {
-    if (a < b) {
-      const int s = a;
-      a = b;
-      b = s;
-    }
-    const int old = atomicCAS(&parent[a], a, b);  // hook the larger root under the smaller
-    if (old == a) return;
-    a = uf_find(parent, old);  // a was hooked elsewhere in the meantime
-    b = uf_find(parent, b);
-  }
-}
-
 // Three (key, triangle) pairs per triangle, edges (a,b), (b,c), (c,a) in that order; key = min*(n_vertices+1) + max,
 // the host's key (mesh.py) and Open3D's GetEdgeToTrianglesMap.  Degenerate edges (a,a) get keys like any other.
 __global__ void __launch_bounds__(256) cluster_edge_keys_kernel(const long long* __restrict__ tris, int nt,
@@ -234,9 +201,7 @@ __global__ void __launch_bounds__(256) cluster_edge_keys_kernel(const long long*
   const long long v[3] = {tris[3 * (size_t)t], tris[3 * (size_t)t + 1], tris[3 * (size_t)t + 2]};
 #pragma unroll
   for (int k = 0; k < 3; ++k) {
-    const long long a = v[k], b = v[(k + 1) % 3];
-    const unsigned long long lo = (unsigned long long)(a < b ? a : b), hi = (unsigned long long)(a < b ? b : a);
-    keys[(size_t)k * nt + t] = lo * stride + hi;
+    keys[(size_t)k * nt + t] = edge_key(v[k], v[(k + 1) % 3], stride);
     owner[(size_t)k * nt + t] = (uint32_t)t;
   }
   parent[t] = t;
@@ -351,12 +316,6 @@ __global__ void clean_sizes_kernel(const int* __restrict__ keep, const int* __re
                                    long long* __restrict__ sizes) {
   sizes[0] = nt ? (long long)tri_pos[nt - 1] + keep[nt - 1] : 0;
   sizes[1] = nv ? (long long)new_id[nv - 1] + referenced[nv - 1] : 0;
-}
-
-inline int bits_of(unsigned long long max_value) {
-  int b = 0;
-  while (b < 64 && (max_value >> b) != 0) ++b;
-  return b;
 }
 
 // Ids are 32-bit inside the kernels; edge keys min*(n_vertices+1) + max then fit 62 bits.

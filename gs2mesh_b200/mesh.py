@@ -8,7 +8,8 @@ does with a hash map).  Connected-component cleaning runs on the GPU for a mesh 
 GPU volume (`TriangleMesh.device` is set) and with numpy / scipy for a mesh built from host arrays;
 both give the same labels, counts and cleaned mesh.  Vertex-clustering simplification (Open3D's
 simplify_vertex_clustering) and the smoothing and sharpening filters (filter_smooth_simple / _laplacian / _taubin,
-filter_sharpen) run on the GPU.  PLY writing stays on the host like in the reference.
+filter_sharpen) run on the GPU, and so do the topology queries (manifoldness, orientability, self-intersection,
+watertightness, Euler characteristic, surface area and volume).  PLY writing stays on the host like in the reference.
 """
 from __future__ import annotations
 
@@ -288,6 +289,69 @@ class TriangleMesh:
             host = lambda a: None if a is None else a.cpu().numpy()
             return type(self)(host(out_v), self.triangles.copy(), host(out_c), host(out_n), device=dev)
 
+    # -- TriangleMesh::GetNonManifoldEdges / IsEdgeManifold / GetNonManifoldVertices / IsVertexManifold /
+    # GetSelfIntersectingTriangles / IsSelfIntersecting / IsOrientable / IsWatertight / EulerPoincareCharacteristic /
+    # GetSurfaceArea / GetVolume (DESIGN.md section 7, "Topology queries").  Each runs on `self.device` (the current CUDA
+    # device for a mesh built from host arrays), returns host values and leaves the mesh unchanged.  ValueError for an
+    # out-of-range triangle index, non-finite vertices or a size past 32-bit ids.
+    def get_non_manifold_edges(self, allow_boundary_edges=True):
+        """int64 (k, 2): the edges (min, max), ascending, with more than two incident triangles, or with
+        allow_boundary_edges=False any count but two.  (a, a, b) puts two incidences on (a, b)."""
+        with _Topology(self) as q:
+            return q.edges(allow_boundary_edges, with_list=True)[0]
+
+    def is_edge_manifold(self, allow_boundary_edges=True):
+        with _Topology(self) as q:
+            return q.edges(allow_boundary_edges)[1] == 0
+
+    def get_non_manifold_vertices(self):
+        """int64 (k,), ascending: the vertices whose link graph (one edge per incident triangle: its first corner pair
+        without the vertex) has more than one component."""
+        with _Topology(self) as q:
+            return q.vertices(with_list=True)[0]
+
+    def is_vertex_manifold(self):
+        with _Topology(self) as q:
+            return q.vertices()[1] == 0
+
+    def get_self_intersecting_triangles(self):
+        """int64 (k, 2), t0 < t1, ascending by (t0, t1): the pairs that share no vertex id, whose boxes overlap and
+        that Open3D's TriangleTriangle3d reports as intersecting."""
+        with _Topology(self) as q:
+            return q.self_intersections(with_list=True)[0]
+
+    def is_self_intersecting(self):
+        with _Topology(self) as q:
+            return q.self_intersections()[1] > 0
+
+    def is_orientable(self):
+        with _Topology(self) as q:
+            return q.edges(True)[3]
+
+    def is_watertight(self):
+        """is_edge_manifold(False) and is_vertex_manifold() and not is_self_intersecting(), on one upload."""
+        with _Topology(self) as q:
+            return q.watertight()
+
+    def euler_poincare_characteristic(self):
+        """V + F - E: every vertex, every triangle, the distinct undirected edges including (a, a)."""
+        with _Topology(self) as q:
+            return len(self.vertices) + len(self.triangles) - q.edges(True)[2]
+
+    def get_surface_area(self):
+        """The sum of 0.5 ||(p0 - p1) x (p0 - p2)|| in a fixed two-stage order."""
+        with _Topology(self) as q:
+            return q.area_volume()[0]
+
+    def get_volume(self):
+        """|sum of p0 . (p1 x p2) / 6|; RuntimeError as Open3D's for a mesh that is not watertight or not orientable."""
+        with _Topology(self) as q:
+            if not q.watertight():
+                raise RuntimeError("The mesh is not watertight, and the volume cannot be computed.")
+            if not q.edges(False)[3]:
+                raise RuntimeError("The mesh is not orientable, and the volume cannot be computed.")
+            return abs(q.area_volume()[1])
+
     # -- o3d.io.write_triangle_mesh(path, mesh): binary little-endian PLY, double coordinates
     def write_ply(self, path):
         nv, nt = len(self.vertices), len(self.triangles)
@@ -315,6 +379,105 @@ class TriangleMesh:
             f.write(vert.tobytes())
             f.write(face.tobytes())
         return path
+
+
+class _Topology:
+    """One upload of a mesh for the topology entries: the checks, the device arrays, and each edge pass's results kept
+    so that is_watertight and get_volume run it once."""
+
+    def __init__(self, mesh):
+        nv, nt = len(mesh.vertices), len(mesh.triangles)
+        if nt and (mesh.triangles.min() < 0 or mesh.triangles.max() >= nv):
+            raise ValueError("topology: triangle vertex index out of range")
+        if not np.isfinite(mesh.vertices).all():
+            raise ValueError("topology: the vertices are not finite")
+        self.mesh, self.nv, self.nt = mesh, nv, nt
+        self.dev = _lib.device(mesh.device)
+        self.L = _lib.lib()
+        self._edges = {}
+        self._xyz = None
+
+    def __enter__(self):
+        self._ctx = torch.cuda.device(self.dev)
+        self._ctx.__enter__()
+        self.stream = _lib.stream(self.dev)
+        self.tri = torch.as_tensor(self.mesh.triangles, dtype=torch.int64).to(self.dev).contiguous()
+        return self
+
+    def __exit__(self, *exc):
+        return self._ctx.__exit__(*exc)
+
+    def _work(self, nbytes):
+        return torch.empty(nbytes, dtype=torch.uint8, device=self.dev)
+
+    def xyz(self):
+        if self._xyz is None:
+            self._xyz = torch.as_tensor(self.mesh.vertices).to(self.dev).contiguous()
+        return self._xyz
+
+    def edges(self, allow_boundary_edges, with_list=False):
+        """(non-manifold edges or None, their count, distinct edges, orientable)."""
+        allow = bool(allow_boundary_edges)
+        if (allow, with_list) not in self._edges and (allow, True) not in self._edges:
+            L = self.L
+            work = self._work(L.gsb_mesh_edge_topology_workspace_bytes(self.nt, self.nv))
+            out = torch.empty(3 * self.nt, 2, dtype=torch.int64, device=self.dev) if with_list else None
+            sizes = torch.empty(3, dtype=torch.int64, device=self.dev)
+            _lib.check(L.gsb_mesh_edge_topology(ptr(self.tri), self.nt, self.nv, int(allow), ptr(work), work.numel(), ptr(out),
+                                                ptr(sizes), self.stream), invalid_is_value_error=True)
+            k, e, orientable = (int(x) for x in sizes.cpu().tolist())
+            self._edges[(allow, with_list)] = (None if out is None else out[:k].cpu().numpy(), k, e, bool(orientable))
+        return self._edges.get((allow, with_list)) or self._edges[(allow, True)]
+
+    def vertices(self, with_list=False):
+        """(non-manifold vertices, their count)."""
+        L = self.L
+        work = self._work(L.gsb_mesh_vertex_topology_workspace_bytes(self.nt, self.nv))
+        out = torch.empty(self.nv, dtype=torch.int64, device=self.dev) if with_list else None
+        count = torch.empty(1, dtype=torch.int64, device=self.dev)
+        _lib.check(L.gsb_mesh_non_manifold_vertices(ptr(self.tri), self.nt, self.nv, ptr(work), work.numel(), ptr(out), ptr(count),
+                                                    self.stream), invalid_is_value_error=True)
+        k = int(count.item())
+        return (out[:k].cpu().numpy() if with_list else None), k
+
+    def self_intersections(self, with_list=False):
+        """(pairs or None, their count); self.stats = (pairs, candidate pairs, registrations, grid level)."""
+        L = self.L
+        v = self.mesh.vertices
+        dbl3 = C.c_double * 3
+        lo = dbl3(*(v.min(axis=0) if self.nv else np.zeros(3)).tolist())
+        hi = dbl3(*(v.max(axis=0) if self.nv else np.zeros(3)).tolist())
+        stats = torch.empty(4, dtype=torch.int64, device=self.dev)
+
+        def run(out, capacity):
+            work = self._work(L.gsb_mesh_self_intersections_workspace_bytes(self.nt, self.nv, capacity))
+            _lib.check(L.gsb_mesh_self_intersections(ptr(self.xyz()), self.nv, ptr(self.tri), self.nt, lo, hi, ptr(work),
+                                                     work.numel(), ptr(out), capacity, ptr(stats), self.stream),
+                       invalid_is_value_error=True)
+            return [int(x) for x in stats.cpu().tolist()]
+
+        self.stats = run(None, 0)
+        k = self.stats[0]
+        if not with_list:
+            return None, k
+        out = torch.empty(k, 2, dtype=torch.int64, device=self.dev)
+        if k:
+            if run(out, k)[0] != k:
+                raise RuntimeError("get_self_intersecting_triangles: the emit pass found a different number of pairs")
+        return out.cpu().numpy(), k
+
+    def watertight(self):
+        return self.edges(False)[1] == 0 and self.vertices()[1] == 0 and self.self_intersections()[1] == 0
+
+    def area_volume(self):
+        """(surface area, signed volume sum)."""
+        L = self.L
+        work = self._work(L.gsb_mesh_area_volume_workspace_bytes(self.nt, self.nv))
+        out = torch.empty(2, dtype=torch.float64, device=self.dev)
+        _lib.check(L.gsb_mesh_area_volume(ptr(self.xyz()), self.nv, ptr(self.tri), self.nt, ptr(work), work.numel(), ptr(out),
+                                          self.stream), invalid_is_value_error=True)
+        a, v = out.cpu().tolist()
+        return a, v
 
 
 def remove_vertices_by_mask(vertices, triangles, vertex_mask, vertex_colors=None, vertex_normals=None):

@@ -28,6 +28,12 @@ and the filters that remove the fused mesh's voxel-scale ripple (each returns a 
     smooth = mesh.filter_smooth_taubin(10)      # also filter_smooth_laplacian, filter_smooth_simple, filter_sharpen
     smooth = mesh.filter_smooth_laplacian(5, 0.5, o3d.geometry.FilterScope.Vertex)
 
+and the topology queries that say whether the result is still a valid surface (host values and numpy arrays):
+
+    mesh.is_watertight(), mesh.is_orientable(), mesh.get_self_intersecting_triangles(), mesh.get_volume()
+    # also get_non_manifold_edges, is_edge_manifold, get_non_manifold_vertices, is_vertex_manifold,
+    # is_self_intersecting, euler_poincare_characteristic, get_surface_area
+
 Differences from Open3D, by construction: the volume lives in GPU memory (an unbounded, hashed set of 16^3 bricks on
 the same voxel lattice, like Open3D's; `window_resolution=` only sets the window dense read-backs look at); images are uploaded on
 integrate().  Everything else (argument names, the RuntimeError on mismatching image sizes, float32 depth

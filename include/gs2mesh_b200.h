@@ -419,6 +419,47 @@ int gsb_mesh_filter(int kind, const double* vertices, const double* colors, cons
                     double param1, int scope, void* workspace, size_t workspace_bytes, double* out_vertices, double* out_colors,
                     double* out_normals, void* stream);
 
+/* Topology queries: TriangleMesh::GetNonManifoldEdges / IsOrientable / EulerPoincareCharacteristic,
+ * GetNonManifoldVertices, GetSelfIntersectingTriangles, GetSurfaceArea and GetVolume of Open3D 0.17.0 (DESIGN.md
+ * section 7, "Topology queries"; restated in tests/topology_oracle.py).  triangles: device int64 [n_triangles,3], every
+ * index in [0, n_vertices) (not checked on the device); vertices: device double [n_vertices,3], finite.  n_triangles <=
+ * 357913941 and n_vertices <= 2^31 - 1 (ids, including the 6 n_triangles link-graph slots, are 32-bit), and a mesh
+ * with triangles has vertices, otherwise GSB_ERR_INVALID.  Each entry takes one caller workspace of its
+ * *_workspace_bytes() (0 for invalid sizes), else GSB_ERR_WORKSPACE; bad arguments are refused before anything is
+ * enqueued; no host sync.
+ *   gsb_mesh_edge_topology  every triangle's edges (0,1), (1,2), (2,0) as incidences of the undirected edge (min, max).
+ *       A non-manifold edge has more than two incidences, or (allow_boundary_edges == 0) any count but two.  out_edges:
+ *       device int64 [3 n_triangles, 2] or NULL: the non-manifold edges as (min, max), ascending.  sizes: device int64
+ *       [3] = (non-manifold edges, distinct edges including (a, a), orientable 0/1).  Orientable: for every edge (a, b),
+ *       a != b, with its incidences in ascending (triangle, corner), each incidence u after the first (c) requires
+ *       flip(u) xor flip(c) = [u and c run a -> b the same way]; the mesh is orientable iff the constraints agree.
+ *   gsb_mesh_non_manifold_vertices  vertex v's link graph has one edge per distinct incident triangle (t0, t1), else
+ *       (t0, t2), else (t1, t2), the first pair without v (none if every pair holds v); v is non-manifold iff the graph
+ *       has more than one component.  out_vertices: device int64 [n_vertices] or NULL (the count only): the non-manifold
+ *       vertices, ascending; count: device int64.
+ *   gsb_mesh_self_intersections  pairs t0 < t1 sharing no vertex id whose boxes overlap (touching included) and that
+ *       pass Moeller's NoDivTriTriIsect (EPSILON 1e-6) on the six points less their mean, divided per axis by
+ *       sqrt(sum of squares / 5) + 1e-12.  min_bound / max_bound: host double[3], the vertices' component-wise min and
+ *       max (they place the grid, not the result).  out_pairs == NULL with capacity 0 counts; else out_pairs: device
+ *       int64 [capacity, 2] receives the pairs ascending by (t0, t1), capacity being the count the first call returned
+ *       (rows past the pairs found are -1).  stats: device int64 [4] = (pairs found, candidate pairs tested, (triangle,
+ *       cell) registrations, grid level: 2^(20 - level) + 1 cells per axis across the largest extent).
+ *   gsb_mesh_area_volume  out: device double [2] = (sum of 0.5 ||(p0 - p1) x (p0 - p2)||, sum of p0 . (p1 x p2) / 6),
+ *       each summed by a fixed two-stage reduction (the same bits on every run). */
+size_t gsb_mesh_edge_topology_workspace_bytes(int64_t n_triangles, int64_t n_vertices);
+int gsb_mesh_edge_topology(const int64_t* triangles, int64_t n_triangles, int64_t n_vertices, int allow_boundary_edges,
+                           void* workspace, size_t workspace_bytes, int64_t* out_edges, int64_t* sizes, void* stream);
+size_t gsb_mesh_vertex_topology_workspace_bytes(int64_t n_triangles, int64_t n_vertices);
+int gsb_mesh_non_manifold_vertices(const int64_t* triangles, int64_t n_triangles, int64_t n_vertices, void* workspace,
+                                   size_t workspace_bytes, int64_t* out_vertices, int64_t* count, void* stream);
+size_t gsb_mesh_self_intersections_workspace_bytes(int64_t n_triangles, int64_t n_vertices, int64_t capacity);
+int gsb_mesh_self_intersections(const double* vertices, int64_t n_vertices, const int64_t* triangles, int64_t n_triangles,
+                                const double* min_bound, const double* max_bound, void* workspace, size_t workspace_bytes,
+                                int64_t* out_pairs, int64_t capacity, int64_t* stats, void* stream);
+size_t gsb_mesh_area_volume_workspace_bytes(int64_t n_triangles, int64_t n_vertices);
+int gsb_mesh_area_volume(const double* vertices, int64_t n_vertices, const int64_t* triangles, int64_t n_triangles,
+                         void* workspace, size_t workspace_bytes, double* out, void* stream);
+
 /* ------------------------------------------------------------------------------------------
  * Point clouds: volume.extract_point_cloud() / extract_voxel_point_cloud()
  * (Open3D ScalableTSDFVolume::ExtractPointCloud / ExtractVoxelPointCloud; DESIGN.md section 7, "Point clouds")
