@@ -443,10 +443,11 @@ class _Topology:
     def self_intersections(self, with_list=False):
         """(pairs or None, their count); self.stats = (pairs, candidate pairs, registrations, grid level)."""
         L = self.L
-        v = self.mesh.vertices
+        # the grid spans the referenced vertices only: a vertex no triangle uses must not stretch the cells
+        v = self.mesh.vertices[self.mesh.triangles.reshape(-1)] if self.nt else np.zeros((1, 3))
         dbl3 = C.c_double * 3
-        lo = dbl3(*(v.min(axis=0) if self.nv else np.zeros(3)).tolist())
-        hi = dbl3(*(v.max(axis=0) if self.nv else np.zeros(3)).tolist())
+        lo = dbl3(*v.min(axis=0).tolist())
+        hi = dbl3(*v.max(axis=0).tolist())
         stats = torch.empty(4, dtype=torch.int64, device=self.dev)
 
         def run(out, capacity):

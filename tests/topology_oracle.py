@@ -137,10 +137,15 @@ def _point_in_tri(V0, U0, U1, U2, i0, i1):
     return (d0 * d1 > 0) & (d0 * d2 > 0)
 
 
+coplanar_axes_hook = None  # called as hook(|N|, i0, i1) by every coplanar test (tests/test_topology_edges_host.py)
+
+
 def _coplanar(N, V0, V1, V2, U0, U1, U2):
     A = np.abs(N)
     i0 = np.where(A[:, 0] > A[:, 1], np.where(A[:, 0] > A[:, 2], 1, 0), 0)
     i1 = np.where(A[:, 0] > A[:, 1], np.where(A[:, 0] > A[:, 2], 2, 1), np.where(A[:, 2] > A[:, 1], 1, 2))
+    if coplanar_axes_hook is not None:
+        coplanar_axes_hook(A, i0, i1)
     return (_edge_against_tri(V0, V1, U0, U1, U2, i0, i1) | _edge_against_tri(V1, V2, U0, U1, U2, i0, i1)
             | _edge_against_tri(V2, V0, U0, U1, U2, i0, i1) | _point_in_tri(V0, U0, U1, U2, i0, i1)
             | _point_in_tri(U0, V0, V1, V2, i0, i1))
@@ -202,10 +207,10 @@ def _no_div_tri_tri(V0, V1, V2, U0, U1, U2):
     return alive & out
 
 
-def tri_tri(P, Q):
-    """TriangleTriangle3d for arrays P, Q (n, 3, 3): the six points less their mean, divided per axis by
-    sqrt(sum of squares / 5) + 1e-12, then NoDivTriTriIsect."""
-    pts = np.concatenate([P, Q], axis=1)  # (n, 6, 3)
+def normalise(P, Q):
+    """TriangleTriangle3d's frame for arrays P, Q (n, 3, 3): the six points (n, 6, 3) less their mean, divided per axis
+    by sqrt(sum of squares / 5) + 1e-12."""
+    pts = np.concatenate([np.asarray(P, np.float64), np.asarray(Q, np.float64)], axis=1)  # (n, 6, 3)
     s = pts[:, 0]
     for k in range(1, 6):
         s = s + pts[:, k]
@@ -214,7 +219,23 @@ def tri_tri(P, Q):
     for k in range(1, 6):
         ss = ss + (pts[:, k] - mu) * (pts[:, k] - mu)
     sigma = np.sqrt(ss / 5.0) + 1e-12
-    q = (pts - mu[:, None]) / sigma[:, None]
+    return (pts - mu[:, None]) / sigma[:, None]
+
+
+def plane_distances(P, Q):
+    """NoDivTriTriIsect's (du, dv) in the normalised frame, before the epsilon clamp: Q's vertices against P's plane and
+    P's against Q's, each (n, 3)."""
+    q = normalise(P, Q)
+    V, U = q[:, :3], q[:, 3:]
+    N1, N2 = _cross(V[:, 1] - V[:, 0], V[:, 2] - V[:, 0]), _cross(U[:, 1] - U[:, 0], U[:, 2] - U[:, 0])
+    d1, d2 = -_dot(N1, V[:, 0]), -_dot(N2, U[:, 0])
+    return (np.stack([_dot(N1, U[:, k]) + d1 for k in range(3)], axis=1),
+            np.stack([_dot(N2, V[:, k]) + d2 for k in range(3)], axis=1))
+
+
+def tri_tri(P, Q):
+    """TriangleTriangle3d for arrays P, Q (n, 3, 3): normalise, then NoDivTriTriIsect."""
+    q = normalise(P, Q)
     return _no_div_tri_tri(*(q[:, k] for k in range(6)))
 
 
