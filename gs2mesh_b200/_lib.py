@@ -124,11 +124,17 @@ SIGNATURES = {
     "gsb_eval_radius_downsample": (C.c_int, [C.POINTER(GsbPointGrid), C.c_double, _vp, _vp, _vp, C.POINTER(C.c_int32), _vp]),
     "gsb_eval_knn": (C.c_int, [C.POINTER(GsbPointGrid), _vp, C.c_int64, C.c_int32, _vp, _vp, _vp]),
     "gsb_eval_estimate_normals": (C.c_int, [C.POINTER(GsbPointGrid), _vp, C.c_int64, C.c_int32, _vp, _vp]),
+    "gsb_pcd_statistical_workspace_bytes": (C.c_size_t, [C.c_int64]),
+    "gsb_pcd_statistical_outliers": (C.c_int, [C.POINTER(GsbPointGrid), C.c_int32, C.c_double, _vp, C.c_size_t, _vp, _vp, _vp,
+                                               _vp]),
+    "gsb_pcd_radius_outliers": (C.c_int, [C.POINTER(GsbPointGrid), C.c_int64, C.c_double, _vp, _vp]),
     "gsb_eval_transform_points": (C.c_int, [_vp, C.c_int64, C.POINTER(C.c_double), _vp, _vp]),
     "gsb_eval_crop_polygon": (C.c_int, [_vp, C.c_int64, _vp, C.c_int32, C.c_int32, C.c_double, C.c_double, _vp, _vp, _vp, _vp]),
     "gsb_eval_voxel_workspace_bytes": (C.c_size_t, [C.c_int64]),
     "gsb_eval_voxel_downsample": (C.c_int, [_vp, C.c_int64, C.POINTER(C.c_double), C.POINTER(C.c_double), C.c_double, _vp,
                                             C.c_size_t, _vp, _vp, _vp]),
+    "gsb_pcd_voxel_downsample": (C.c_int, [_vp, _vp, _vp, C.c_int64, C.POINTER(C.c_double), C.POINTER(C.c_double), C.c_double,
+                                           _vp, C.c_size_t, _vp, _vp, _vp, _vp, _vp]),
     "gsb_eval_icp_correspond": (C.c_int, [C.POINTER(GsbPointGrid), _vp, C.c_int64, C.c_double, _vp, _vp, _vp]),
     "gsb_eval_icp_moments": (C.c_int, [_vp, _vp, _vp, C.c_int64, _vp, C.c_int, C.POINTER(C.c_double), _vp, _vp, _vp]),
     "gsb_eval_mask_dilate_disk":(C.c_int, [_vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _vp, _vp, _vp]),

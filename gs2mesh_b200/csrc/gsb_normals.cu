@@ -1,6 +1,7 @@
 // Exact k nearest neighbours on the shared point grid, and Open3D 0.17's PointCloud::EstimateNormals with
 // KDTreeSearchParamKNN(k) and fast_normal_computation (ComputeCovariance, FastEigen3x3) for a cloud without normals: the
-// Tanks and Temples toolbox's estimate_normals (evaluation.py:60-84).
+// Tanks and Temples toolbox's estimate_normals (evaluation.py:60-84).  Open3D 0.17's PointCloud::RemoveStatisticalOutliers
+// and RemoveRadiusOutliers on the same grid (DESIGN.md section 7, "Point-cloud cleaning and downsampling").
 //
 // Every fp64 operation carries an explicit rounding intrinsic, so nvcc cannot contract a multiply-add into an FMA, and
 // acos / cos are fdlibm's algorithms in those operations rather than the device's libm: tests/normals_oracle.py restates
@@ -301,6 +302,83 @@ __global__ void __launch_bounds__(128, 4) normals_kernel(const GsbPointGrid g, c
   out[3 * t + 2] = nrm.z;
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// RemoveStatisticalOutliers: m_i = (((0.0 + sqrt(d2_0)) + sqrt(d2_1)) + ...) / double(c) over the c = min(k, n) nearest
+// grid points of grid point i (itself included), then mean and standard deviation of the positive m_i by a fixed-order
+// sum S (chunks of kStatChunk consecutive indices summed sequentially from 0.0, then the chunk sums sequentially from
+// 0.0), so every run writes the same bytes.  A skipped term adds nothing: a sum from +0.0 of values >= 0 is never -0.0,
+// so skipping equals adding +0.0.
+// ---------------------------------------------------------------------------------------------------------------------
+constexpr int kStatChunk = 1024;
+
+__global__ void __launch_bounds__(128, 4) stat_mean_kernel(const GsbPointGrid g, int k, double* __restrict__ mean_dist) {
+  const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= g.n_points) return;
+  double d2s[kMaxK];
+  long long ids[kMaxK];
+  const double* p = g.points + 3 * t;
+  const int c = ring_knn(g, p[0], p[1], p[2], k, d2s, ids);
+  double s = 0.0;
+  for (int j = 0; j < c; ++j) s = add(s, __dsqrt_rn(d2s[j]));
+  mean_dist[t] = quo(s, (double)c);
+}
+
+// pass 0: the chunk sums of m_i over m_i > 0; pass 1: of (m_i - mean) * (m_i - mean) over m_i > 0, mean = stats[0]
+__global__ void __launch_bounds__(128) stat_chunk_kernel(const double* __restrict__ mean_dist, long long n, int pass,
+                                                         const double* __restrict__ stats, double* __restrict__ partial) {
+  const long long c = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (c * kStatChunk >= n) return;
+  const double mean = pass ? stats[0] : 0.0;
+  const long long e = min(n, (c + 1) * kStatChunk);
+  double s = 0.0;
+  for (long long i = c * kStatChunk; i < e; ++i) {
+    const double m = mean_dist[i];
+    if (m > 0.0) s = add(s, pass ? mul(sub(m, mean), sub(m, mean)) : m);
+  }
+  partial[c] = s;
+}
+
+// One thread: the chunk sums in chunk order.  pass 0 writes stats[0] = S / double(n); pass 1 writes stats[1] =
+// sqrt(S / double(n - 1)) and stats[2] = mean + std_ratio * std.
+__global__ void stat_total_kernel(const double* __restrict__ partial, long long n, int pass, double std_ratio,
+                                  double* __restrict__ stats) {
+  const long long chunks = (n + kStatChunk - 1) / kStatChunk;
+  double s = 0.0;
+  for (long long c = 0; c < chunks; ++c) s = add(s, partial[c]);
+  if (pass == 0) {
+    stats[0] = quo(s, (double)n);
+  } else {
+    const double sd = __dsqrt_rn(quo(s, (double)(n - 1)));
+    stats[1] = sd;
+    stats[2] = add(stats[0], mul(std_ratio, sd));
+  }
+}
+
+__global__ void __launch_bounds__(256) stat_keep_kernel(const double* __restrict__ mean_dist, long long n,
+                                                        const double* __restrict__ stats, uint8_t* __restrict__ keep) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const double m = mean_dist[i];
+  keep[i] = m > 0.0 && m < stats[2];
+}
+
+// RemoveRadiusOutliers: keep[i] = 1 iff more than nb_points grid points j (i itself included) have
+// ((dx*dx)+dy*dy)+dz*dz < r2, strictly (nanoflann's radius result set).  The 27-cell walk stops once the count passes
+// nb_points; a point with a non-finite coordinate is not kept.
+__global__ void __launch_bounds__(256) radius_outlier_kernel(const GsbPointGrid g, long long nb_points, double r2,
+                                                             uint8_t* __restrict__ keep) {
+  const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= g.n_points) return;
+  const double x = g.points[3 * t], y = g.points[3 * t + 1], z = g.points[3 * t + 2];
+  long long count = 0;
+  if (isfinite(x) && isfinite(y) && isfinite(z))
+    visit_27_cells(g, x, y, z, [&](long long q) {
+      count += sq_dist(x, y, z, g.points + 3 * q) < r2;
+      return count <= nb_points;
+    });
+  keep[t] = count > nb_points;
+}
+
 }  // namespace
 }  // namespace gsb
 
@@ -329,6 +407,46 @@ int gsb_eval_estimate_normals(const GsbPointGrid* grid, const double* points, in
   normals_kernel<<<blocks_for(n_points, 128), 128, 0, stream>>>(*grid, points, n_points, k, normals);
   count_launch();
   return check_launch("normals_kernel", stream, false);
+}
+
+size_t gsb_pcd_statistical_workspace_bytes(int64_t n_points) {
+  if (n_points < 0 || n_points > 2147483647) return 0;
+  return align_up(sizeof(double) * (size_t)((n_points + kStatChunk - 1) / kStatChunk), 256);
+}
+
+int gsb_pcd_statistical_outliers(const GsbPointGrid* grid, int32_t k, double std_ratio, void* workspace,
+                                 size_t workspace_bytes, double* mean_dist, uint8_t* keep, double* stats, void* stream_v) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
+  if (!grid_ok(grid) || grid->n_points > 2147483647 || k < 1 || k > kMaxK || !(std_ratio > 0.0) ||
+      (grid->n_points && (!workspace || !mean_dist || !keep || !stats)))
+    return fail(GSB_ERR_INVALID, "pcd_statistical_outliers: bad arguments (k must be in 1..%d, std_ratio > 0)", kMaxK);
+  const long long n = grid->n_points;
+  if (n == 0) return GSB_OK;
+  if (workspace_bytes < gsb_pcd_statistical_workspace_bytes(n))
+    return fail(GSB_ERR_WORKSPACE, "pcd_statistical_outliers: workspace %zu < %zu bytes", workspace_bytes,
+                gsb_pcd_statistical_workspace_bytes(n));
+  double* partial = static_cast<double*>(workspace);
+  const long long chunks = (n + kStatChunk - 1) / kStatChunk;
+  stat_mean_kernel<<<blocks_for(n, 128), 128, 0, stream>>>(*grid, k, mean_dist);
+  for (int pass = 0; pass < 2; ++pass) {
+    stat_chunk_kernel<<<blocks_for(chunks, 128), 128, 0, stream>>>(mean_dist, n, pass, stats, partial);
+    stat_total_kernel<<<1, 1, 0, stream>>>(partial, n, pass, std_ratio, stats);
+  }
+  stat_keep_kernel<<<blocks_for(n), 256, 0, stream>>>(mean_dist, n, stats, keep);
+  count_launch(6);
+  return check_launch("statistical outliers", stream, false);
+}
+
+int gsb_pcd_radius_outliers(const GsbPointGrid* grid, int64_t nb_points, double radius, uint8_t* keep, void* stream_v) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
+  if (!grid_ok(grid) || nb_points < 1 || !(radius > 0.0) || !(radius < INFINITY) || (grid->n_points && !keep) ||
+      !(grid->cell >= radius * 1.0000001))
+    return fail(GSB_ERR_INVALID,
+                "pcd_radius_outliers: bad arguments (nb_points >= 1, a finite radius > 0, the grid cell above the radius)");
+  if (grid->n_points == 0) return GSB_OK;
+  radius_outlier_kernel<<<blocks_for(grid->n_points), 256, 0, stream>>>(*grid, nb_points, radius * radius, keep);
+  count_launch();
+  return check_launch("radius_outlier_kernel", stream, false);
 }
 
 }  // extern "C"

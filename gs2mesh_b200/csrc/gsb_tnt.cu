@@ -96,18 +96,22 @@ __global__ void __launch_bounds__(256) voxel_head_kernel(const unsigned long lon
   if (i < n) head[i] = i == 0 || keys[i] != keys[i - 1];
 }
 
-__global__ void __launch_bounds__(256) voxel_mean_kernel(const double* __restrict__ pts, long long n,
+// The mean of each voxel's values v (points, colours or normals) in input order from 0.0, divided by the voxel's point
+// count.  With skip_nan a row with a NaN component adds nothing but still counts (Open3D's AccumulatedPoint normal).
+__global__ void __launch_bounds__(256) voxel_mean_kernel(const double* __restrict__ v, long long n,
                                                          const long long* __restrict__ ids, const long long* __restrict__ starts,
-                                                         const long long* __restrict__ n_voxels, double* __restrict__ out) {
+                                                         const long long* __restrict__ n_voxels, bool skip_nan,
+                                                         double* __restrict__ out) {
   const long long vx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   const long long nv = *n_voxels;
   if (vx >= nv) return;
   const long long s = starts[vx], e = vx + 1 < nv ? starts[vx + 1] : n;
   double sum[3] = {0.0, 0.0, 0.0};
   for (long long k = s; k < e; ++k) {
-    const long long id = ids[k];
+    const double* r = v + 3 * ids[k];
+    if (skip_nan && (isnan(r[0]) || isnan(r[1]) || isnan(r[2]))) continue;
 #pragma unroll
-    for (int a = 0; a < 3; ++a) sum[a] = __dadd_rn(sum[a], pts[3 * id + a]);
+    for (int a = 0; a < 3; ++a) sum[a] = __dadd_rn(sum[a], r[a]);
   }
   const double cnt = (double)(e - s);
 #pragma unroll
@@ -215,6 +219,87 @@ bool host_finite(const double* v, int n) {
   return true;
 }
 
+size_t voxel_workspace_bytes(int64_t n_points) {
+  if (n_points < 0 || n_points >= 2147483647) return 0;
+  const int n = (int)n_points;
+  size_t sort_bytes = 0, select_bytes = 0;
+  cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, (unsigned long long*)nullptr, (unsigned long long*)nullptr,
+                                  (long long*)nullptr, (long long*)nullptr, n);
+  cub::DeviceSelect::Flagged(nullptr, select_bytes, cub::CountingInputIterator<long long>(0), (uint8_t*)nullptr,
+                             (long long*)nullptr, (long long*)nullptr, n);
+  Carver c(nullptr);
+  c.take<unsigned long long>(2 * (size_t)n);
+  c.take<long long>(3 * (size_t)n);
+  c.take<uint8_t>((size_t)n);
+  c.take<char>(sort_bytes > select_bytes ? sort_bytes : select_bytes);
+  return c.total();
+}
+
+// gsb_eval_voxel_downsample and gsb_pcd_voxel_downsample: keys, stable sort, voxel heads, their starts, then the mean of
+// the points and of the colours and normals that are given.  `who` prefixes the messages.
+int voxel_downsample(const char* who, const double* points, const double* colors, const double* normals, int64_t n_points,
+                     const double* min_bound, const double* max_bound, double voxel_size, void* workspace,
+                     size_t workspace_bytes, double* out, double* out_colors, double* out_normals, int64_t* n_out,
+                     cudaStream_t stream) {
+  if (n_points < 0 || n_points >= 2147483647 || !(voxel_size > 0.0) || !(voxel_size < INFINITY) || !min_bound || !max_bound ||
+      !n_out || (n_points && (!points || !out || !workspace)))
+    return fail(GSB_ERR_INVALID, "%s: bad arguments", who);
+  if (n_points == 0) {
+    GSB_CUDA_OK(cudaMemsetAsync(n_out, 0, sizeof(int64_t), stream));
+    return GSB_OK;
+  }
+  if (!host_finite(min_bound, 3) || !host_finite(max_bound, 3))
+    return fail(GSB_ERR_INVALID, "%s: the points are not finite", who);
+  VoxelGrid g;
+  g.voxel = voxel_size;
+  double span = 0.0;
+  for (int a = 0; a < 3; ++a) {
+    g.lo[a] = min_bound[a] - voxel_size * 0.5;
+    span = std::max(span, (max_bound[a] + voxel_size * 0.5) - g.lo[a]);
+  }
+  if (voxel_size * 2147483647.0 < span)  // Open3D: voxel_size * INT_MAX < (voxel_max_bound - voxel_min_bound).maxCoeff()
+    return fail(GSB_ERR_INVALID, "%s: voxel_size is too small (voxel_size * INT_MAX < %g)", who, span);
+  long long extent[3];  // voxels per axis; the largest index is that of max_bound
+  for (int a = 0; a < 3; ++a) extent[a] = (long long)std::floor((max_bound[a] - g.lo[a]) / voxel_size) + 1;
+  const int bx = bits_for(extent[0]), by = bits_for(extent[1]), bz = bits_for(extent[2]);
+  if (bx + by + bz > 63)
+    return fail(GSB_ERR_INVALID,
+                "%s: %lld x %lld x %lld voxels need %d key bits; voxel keys are limited to 63 bits", who,
+                extent[0], extent[1], extent[2], bx + by + bz);
+  g.shift_x = by + bz;
+  g.shift_y = bz;
+  if (workspace_bytes < voxel_workspace_bytes(n_points))
+    return fail(GSB_ERR_WORKSPACE, "%s: workspace %zu < %zu bytes", who, workspace_bytes,
+                voxel_workspace_bytes(n_points));
+  const int n = (int)n_points;
+  Carver c(workspace);
+  unsigned long long* keys = c.take<unsigned long long>(2 * (size_t)n);
+  long long* ids = c.take<long long>(3 * (size_t)n);
+  uint8_t* head = c.take<uint8_t>((size_t)n);
+  size_t tmp_bytes = workspace_bytes - c.total();
+  void* tmp = c.take<char>(tmp_bytes);
+  voxel_key_kernel<<<blocks_for(n), 256, 0, stream>>>(points, n, g, keys, ids);
+  count_launch();
+  GSB_CUDA_OK(cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, keys, keys + n, ids, ids + n, n, 0, bx + by + bz, stream));
+  voxel_head_kernel<<<blocks_for(n), 256, 0, stream>>>(keys + n, n, head);
+  count_launch();
+  long long* starts = ids + 2 * (size_t)n;
+  auto* n_voxels = reinterpret_cast<long long*>(n_out);
+  GSB_CUDA_OK(cub::DeviceSelect::Flagged(tmp, tmp_bytes, cub::CountingInputIterator<long long>(0), head, starts, n_voxels, n,
+                                         stream));
+  voxel_mean_kernel<<<blocks_for(n), 256, 0, stream>>>(points, n, ids + n, starts, n_voxels, false, out);
+  count_launch();
+  if (colors) {
+    voxel_mean_kernel<<<blocks_for(n), 256, 0, stream>>>(colors, n, ids + n, starts, n_voxels, false, out_colors);
+    count_launch();
+  }
+  if (normals) {
+    voxel_mean_kernel<<<blocks_for(n), 256, 0, stream>>>(normals, n, ids + n, starts, n_voxels, true, out_normals);
+    count_launch();
+  }
+  return check_launch("voxel downsample", stream, false);
+}
+
 }  // namespace
 }  // namespace gsb
 
@@ -259,75 +344,24 @@ int gsb_eval_crop_polygon(const double* points, int64_t n_points, const double* 
   return GSB_OK;
 }
 
-size_t gsb_eval_voxel_workspace_bytes(int64_t n_points) {
-  if (n_points < 0 || n_points >= 2147483647) return 0;
-  const int n = (int)n_points;
-  size_t sort_bytes = 0, select_bytes = 0;
-  cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, (unsigned long long*)nullptr, (unsigned long long*)nullptr,
-                                  (long long*)nullptr, (long long*)nullptr, n);
-  cub::DeviceSelect::Flagged(nullptr, select_bytes, cub::CountingInputIterator<long long>(0), (uint8_t*)nullptr,
-                             (long long*)nullptr, (long long*)nullptr, n);
-  Carver c(nullptr);
-  c.take<unsigned long long>(2 * (size_t)n);
-  c.take<long long>(3 * (size_t)n);
-  c.take<uint8_t>((size_t)n);
-  c.take<char>(sort_bytes > select_bytes ? sort_bytes : select_bytes);
-  return c.total();
-}
+size_t gsb_eval_voxel_workspace_bytes(int64_t n_points) { return voxel_workspace_bytes(n_points); }
 
 int gsb_eval_voxel_downsample(const double* points, int64_t n_points, const double* min_bound, const double* max_bound,
                               double voxel_size, void* workspace, size_t workspace_bytes, double* out, int64_t* n_out,
                               void* stream_v) {
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
-  if (n_points < 0 || n_points >= 2147483647 || !(voxel_size > 0.0) || !(voxel_size < INFINITY) || !min_bound || !max_bound ||
-      !n_out || (n_points && (!points || !out || !workspace)))
-    return fail(GSB_ERR_INVALID, "eval_voxel_downsample: bad arguments");
-  if (n_points == 0) {
-    GSB_CUDA_OK(cudaMemsetAsync(n_out, 0, sizeof(int64_t), stream));
-    return GSB_OK;
-  }
-  if (!host_finite(min_bound, 3) || !host_finite(max_bound, 3))
-    return fail(GSB_ERR_INVALID, "eval_voxel_downsample: the points are not finite");
-  VoxelGrid g;
-  g.voxel = voxel_size;
-  double span = 0.0;
-  for (int a = 0; a < 3; ++a) {
-    g.lo[a] = min_bound[a] - voxel_size * 0.5;
-    span = std::max(span, (max_bound[a] + voxel_size * 0.5) - g.lo[a]);
-  }
-  if (voxel_size * 2147483647.0 < span)  // Open3D: voxel_size * INT_MAX < (voxel_max_bound - voxel_min_bound).maxCoeff()
-    return fail(GSB_ERR_INVALID, "eval_voxel_downsample: voxel_size is too small (voxel_size * INT_MAX < %g)", span);
-  long long extent[3];  // voxels per axis; the largest index is that of max_bound
-  for (int a = 0; a < 3; ++a) extent[a] = (long long)std::floor((max_bound[a] - g.lo[a]) / voxel_size) + 1;
-  const int bx = bits_for(extent[0]), by = bits_for(extent[1]), bz = bits_for(extent[2]);
-  if (bx + by + bz > 63)
-    return fail(GSB_ERR_INVALID,
-                "eval_voxel_downsample: %lld x %lld x %lld voxels need %d key bits; voxel keys are limited to 63 bits",
-                extent[0], extent[1], extent[2], bx + by + bz);
-  g.shift_x = by + bz;
-  g.shift_y = bz;
-  if (workspace_bytes < gsb_eval_voxel_workspace_bytes(n_points))
-    return fail(GSB_ERR_WORKSPACE, "eval_voxel_downsample: workspace %zu < %zu bytes", workspace_bytes,
-                gsb_eval_voxel_workspace_bytes(n_points));
-  const int n = (int)n_points;
-  Carver c(workspace);
-  unsigned long long* keys = c.take<unsigned long long>(2 * (size_t)n);
-  long long* ids = c.take<long long>(3 * (size_t)n);
-  uint8_t* head = c.take<uint8_t>((size_t)n);
-  size_t tmp_bytes = workspace_bytes - c.total();
-  void* tmp = c.take<char>(tmp_bytes);
-  voxel_key_kernel<<<blocks_for(n), 256, 0, stream>>>(points, n, g, keys, ids);
-  count_launch();
-  GSB_CUDA_OK(cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, keys, keys + n, ids, ids + n, n, 0, bx + by + bz, stream));
-  voxel_head_kernel<<<blocks_for(n), 256, 0, stream>>>(keys + n, n, head);
-  count_launch();
-  long long* starts = ids + 2 * (size_t)n;
-  auto* n_voxels = reinterpret_cast<long long*>(n_out);
-  GSB_CUDA_OK(cub::DeviceSelect::Flagged(tmp, tmp_bytes, cub::CountingInputIterator<long long>(0), head, starts, n_voxels, n,
-                                         stream));
-  voxel_mean_kernel<<<blocks_for(n), 256, 0, stream>>>(points, n, ids + n, starts, n_voxels, out);
-  count_launch();
-  return check_launch("voxel downsample", stream, false);
+  return voxel_downsample("eval_voxel_downsample", points, nullptr, nullptr, n_points, min_bound, max_bound, voxel_size,
+                          workspace, workspace_bytes, out, nullptr, nullptr, n_out, static_cast<cudaStream_t>(stream_v));
+}
+
+int gsb_pcd_voxel_downsample(const double* points, const double* colors, const double* normals, int64_t n_points,
+                             const double* min_bound, const double* max_bound, double voxel_size, void* workspace,
+                             size_t workspace_bytes, double* out, double* out_colors, double* out_normals, int64_t* n_out,
+                             void* stream_v) {
+  if (!colors != !out_colors || !normals != !out_normals)
+    return fail(GSB_ERR_INVALID, "pcd_voxel_downsample: colours and normals need both their input and their output");
+  return voxel_downsample("pcd_voxel_downsample", points, colors, normals, n_points, min_bound, max_bound, voxel_size,
+                          workspace, workspace_bytes, out, out_colors, out_normals, n_out,
+                          static_cast<cudaStream_t>(stream_v));
 }
 
 int gsb_eval_icp_moments(const double* source, const int64_t* index, const double* dist2, int64_t n_source,

@@ -9,7 +9,10 @@ GPU volume (`TriangleMesh.device` is set) and with numpy / scipy for a mesh buil
 both give the same labels, counts and cleaned mesh.  Vertex-clustering simplification (Open3D's
 simplify_vertex_clustering) and the smoothing and sharpening filters (filter_smooth_simple / _laplacian / _taubin,
 filter_sharpen) run on the GPU, and so do the topology queries (manifoldness, orientability, self-intersection,
-watertightness, Euler characteristic, surface area and volume).  PLY writing stays on the host like in the reference.
+watertightness, Euler characteristic, surface area and volume).  The extracted PointCloud is cleaned and thinned on the GPU
+too (gs2mesh_b200/pointcloud.py): remove_statistical_outlier, remove_radius_outlier, select_by_index, voxel_down_sample
+with colours and normals, uniform_down_sample, compute_nearest_neighbor_distance and compute_point_cloud_distance.  PLY
+writing stays on the host like in the reference.
 """
 from __future__ import annotations
 
@@ -21,6 +24,7 @@ import numpy as np
 import torch
 
 from . import _lib
+from . import pointcloud as _pcd
 from ._lib import ptr
 
 
@@ -565,6 +569,42 @@ class PointCloud:
         c = np.asarray(center, dtype=np.float64)
         self.points = (self.points - c) * float(scale) + c
         return self
+
+    # -- PointCloud::RemoveStatisticalOutliers / RemoveRadiusOutliers / SelectByIndex / VoxelDownSample /
+    # UniformDownSample / ComputeNearestNeighborDistance / ComputePointCloudDistance (DESIGN.md section 7, "Point-cloud
+    # cleaning and downsampling"; gs2mesh_b200/pointcloud.py).  Each runs on `self.device` (the current CUDA device for a
+    # cloud built from host arrays), returns a new cloud of the same class holding host arrays with that device set, or
+    # host values, and leaves the cloud unchanged; colours and normals travel with their points.  ValueError for
+    # non-finite points, a colour or normal array without one row per point, or 2^31 points or more.
+    def remove_statistical_outlier(self, nb_neighbors, std_ratio, print_progress=False):
+        """(cloud, int64 indices ascending): keeps point i iff its mean distance m_i to its nb_neighbors nearest points
+        (itself included) satisfies 0 < m_i < mean + std_ratio * std of the positive m_i over the cloud's n points."""
+        return _pcd.remove_statistical_outlier(self, nb_neighbors, std_ratio)
+
+    def remove_radius_outlier(self, nb_points, radius, print_progress=False):
+        """(cloud, int64 indices ascending): keeps point i iff more than nb_points points (itself included) lie at squared
+        distance strictly below radius * radius."""
+        return _pcd.remove_radius_outlier(self, nb_points, radius)
+
+    def select_by_index(self, indices, invert=False):
+        """The points at `indices` (or, with invert, the others) in ascending index order, each once."""
+        return _pcd.select_by_index(self, indices, invert)
+
+    def voxel_down_sample(self, voxel_size):
+        """The mean point, colour and normal of each occupied voxel, in ascending (x, y, z) voxel order."""
+        return _pcd.voxel_down_sample(self, voxel_size)
+
+    def uniform_down_sample(self, every_k_points):
+        """Points 0, k, 2k, ... with their colours and normals."""
+        return _pcd.uniform_down_sample(self, every_k_points)
+
+    def compute_nearest_neighbor_distance(self):
+        """fp64 numpy (n,): each point's distance to its nearest other point."""
+        return _pcd.compute_nearest_neighbor_distance(self)
+
+    def compute_point_cloud_distance(self, target):
+        """fp64 numpy (n,): each point's distance to the nearest point of `target`."""
+        return _pcd.compute_point_cloud_distance(self, target)
 
     # -- o3d.io.write_point_cloud(path, pcd): binary little-endian PLY, double coordinates and normals, uchar colours
     def write_ply(self, path):

@@ -34,6 +34,13 @@ and the topology queries that say whether the result is still a valid surface (h
     # also get_non_manifold_edges, is_edge_manifold, get_non_manifold_vertices, is_vertex_manifold,
     # is_self_intersecting, euler_poincare_characteristic, get_surface_area
 
+and the cleaning and thinning of the extracted cloud (each returns a new cloud; indices are int64 numpy arrays):
+
+    clean, ind = pcd.remove_statistical_outlier(nb_neighbors=20, std_ratio=2.0)
+    clean, ind = pcd.remove_radius_outlier(nb_points=16, radius=0.05)
+    thin = clean.voxel_down_sample(voxel_size=0.01)          # colours and normals averaged
+    # also select_by_index, uniform_down_sample, compute_nearest_neighbor_distance, compute_point_cloud_distance
+
 Differences from Open3D, by construction: the volume lives in GPU memory (an unbounded, hashed set of 16^3 bricks on
 the same voxel lattice, like Open3D's; `window_resolution=` only sets the window dense read-backs look at); images are uploaded on
 integrate().  Everything else (argument names, the RuntimeError on mismatching image sizes, float32 depth

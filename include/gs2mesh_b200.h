@@ -550,7 +550,8 @@ int gsb_eval_grid_build(const GsbPointGrid* grid, void* workspace, size_t worksp
 int gsb_eval_nearest(const GsbPointGrid* grid, const double* queries, int64_t n_queries, double max_dist, double* dist,
                      int64_t* index, void* stream);
 /* Greedy radius downsampling of the grid's points in index order (eval.py:88-93): keep[p] = 1 iff no earlier kept point q
- * has ((dx*dx)+dy*dy)+dz*dz <= radius*radius (sklearn radius_neighbors, inclusive).  Needs grid->cell > radius.
+ * has ((dx*dx)+dy*dy)+dz*dz <= radius*radius (sklearn radius_neighbors, inclusive; gsb_pcd_radius_outliers' test is
+ * strict, as nanoflann's).  Needs grid->cell > radius.
  * Runs rounds of the parallel greedy rule and reads the undecided count every 4 rounds: SYNCHRONISES the stream.
  * keep: device uint8[n_points]; counters: device uint32[4] scratch; host_undecided: pinned host uint32[1];
  * rounds (may be NULL) receives the number of rounds run. */
@@ -576,6 +577,26 @@ int gsb_eval_knn(const GsbPointGrid* grid, const double* queries, int64_t n_quer
                  int64_t* index, void* stream);
 int gsb_eval_estimate_normals(const GsbPointGrid* grid, const double* points, int64_t n_points, int32_t k, double* normals,
                               void* stream);
+
+/* Point-cloud cleaning: Open3D 0.17's PointCloud::RemoveStatisticalOutliers and RemoveRadiusOutliers over the grid's own
+ * points (gsb_normals.cu; DESIGN.md section 7, "Point-cloud cleaning and downsampling"; restated in tests/pcd_oracle.py).
+ * The grid's points must be finite and fewer than 2^31.  Bad arguments are refused (GSB_ERR_INVALID) before anything is
+ * enqueued; a grid without points enqueues nothing.  No allocation, no host sync; every run writes the same bytes.
+ *   gsb_pcd_statistical_outliers  mean_dist[i] (device double [n]) = (((0.0 + sqrt(d2_0)) + sqrt(d2_1)) + ...) / double(c)
+ *       over the c = min(k, n) nearest grid points of point i in gsb_eval_knn's order (itself included), 1 <= k <=
+ *       GSB_KNN_MAX_K.  S is a fixed-order sum: chunks of 1024 consecutive indices, each summed sequentially from 0.0,
+ *       then the chunk sums sequentially from 0.0.  stats (device double [3]) = (mean = S(m_i : m_i > 0) / double(n),
+ *       std = sqrt(S((m_i - mean) * (m_i - mean) : m_i > 0) / double(n - 1)), thr = mean + std_ratio * std), NaN for
+ *       n = 1.  keep[i] (device uint8 [n]) = m_i > 0 and m_i < thr.  std_ratio > 0 (not NaN).  One caller workspace of
+ *       gsb_pcd_statistical_workspace_bytes(n) (0 for invalid sizes), else GSB_ERR_WORKSPACE.
+ *   gsb_pcd_radius_outliers  keep[i] = 1 iff more than nb_points grid points j (i included) have
+ *       ((dx*dx)+dy*dy)+dz*dz < radius*radius, strictly (the sum rounded per operation, radius*radius rounded once;
+ *       gsb_eval_radius_downsample's test is inclusive).  nb_points >= 1, radius finite and > 0, and the grid cell at least
+ *       radius * 1.0000001.  Each point's search stops once its count passes nb_points. */
+size_t gsb_pcd_statistical_workspace_bytes(int64_t n_points);
+int gsb_pcd_statistical_outliers(const GsbPointGrid* grid, int32_t k, double std_ratio, void* workspace,
+                                 size_t workspace_bytes, double* mean_dist, uint8_t* keep, double* stats, void* stream);
+int gsb_pcd_radius_outliers(const GsbPointGrid* grid, int64_t nb_points, double radius, uint8_t* keep, void* stream);
 
 /* Tanks and Temples evaluation (evaluation/TNT/eval_code/python_toolbox/evaluation), restating Open3D 0.17's
  * PointCloud::Transform, SelectionPolygonVolume::CropInPolygon, VoxelDownSample and RegistrationICP with
@@ -612,6 +633,16 @@ size_t gsb_eval_voxel_workspace_bytes(int64_t n_points);
 int gsb_eval_voxel_downsample(const double* points, int64_t n_points, const double* min_bound, const double* max_bound,
                               double voxel_size, void* workspace, size_t workspace_bytes, double* out, int64_t* n_out,
                               void* stream);
+/* PointCloud::VoxelDownSample with colours and normals (DESIGN.md section 7, "Point-cloud cleaning and downsampling"):
+ * gsb_eval_voxel_downsample's voxels, order, points and refusals, with the same workspace
+ * (gsb_eval_voxel_workspace_bytes).  colors / normals: device double [n_points,3] or NULL, each given together with its
+ * output out_colors / out_normals (device double [n_points,3]), else GSB_ERR_INVALID.  Each voxel's colour and normal is
+ * the sum over its points in input order from 0.0, divided by double(the voxel's point count); a normal with a NaN
+ * component adds nothing but its point still counts (Open3D's AccumulatedPoint).  Normals are not renormalised. */
+int gsb_pcd_voxel_downsample(const double* points, const double* colors, const double* normals, int64_t n_points,
+                             const double* min_bound, const double* max_bound, double voxel_size, void* workspace,
+                             size_t workspace_bytes, double* out, double* out_colors, double* out_normals, int64_t* n_out,
+                             void* stream);
 int gsb_eval_icp_correspond(const GsbPointGrid* grid, const double* source, int64_t n_source, double radius, int64_t* index,
                             double* dist2, void* stream);
 int gsb_eval_icp_moments(const double* source, const int64_t* index, const double* dist2, int64_t n_source,
