@@ -131,8 +131,6 @@ SIGNATURES = {
     "gsb_eval_transform_points": (C.c_int, [_vp, C.c_int64, C.POINTER(C.c_double), _vp, _vp]),
     "gsb_eval_crop_polygon": (C.c_int, [_vp, C.c_int64, _vp, C.c_int32, C.c_int32, C.c_double, C.c_double, _vp, _vp, _vp, _vp]),
     "gsb_eval_voxel_workspace_bytes": (C.c_size_t, [C.c_int64]),
-    "gsb_eval_voxel_downsample": (C.c_int, [_vp, C.c_int64, C.POINTER(C.c_double), C.POINTER(C.c_double), C.c_double, _vp,
-                                            C.c_size_t, _vp, _vp, _vp]),
     "gsb_pcd_voxel_downsample": (C.c_int, [_vp, _vp, _vp, C.c_int64, C.POINTER(C.c_double), C.POINTER(C.c_double), C.c_double,
                                            _vp, C.c_size_t, _vp, _vp, _vp, _vp, _vp]),
     "gsb_eval_icp_correspond": (C.c_int, [C.POINTER(GsbPointGrid), _vp, C.c_int64, C.c_double, _vp, _vp, _vp]),

@@ -124,6 +124,24 @@ inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 // blocks of `threads` threads that cover n items
 inline unsigned blocks_for(long long n, int threads = 256) { return (unsigned)((n + threads - 1) / threads); }
 
+// Mesh entries index vertices and triangles with 32-bit ids.  A mesh they accept has non-negative sizes, no triangles
+// without vertices, at most kMaxMeshIds vertices and at most max_triangles triangles (kMaxMeshIds, or fewer where an entry
+// keeps several ids per triangle).  mesh_size_error gives the refusal of a mesh mesh_sizes_ok rejects, prefixed `who: `.
+constexpr int64_t kMaxMeshIds = 2147483647;
+
+inline bool mesh_sizes_ok(int64_t nt, int64_t nv, int64_t max_triangles) {
+  return nt >= 0 && nv >= 0 && nt <= max_triangles && nv <= kMaxMeshIds && (nt == 0 || nv > 0);
+}
+
+inline int mesh_size_error(const char* who, int64_t nt, int64_t nv, int64_t max_triangles) {
+  if (nt < 0 || nv < 0)
+    return fail(GSB_ERR_INVALID, "%s: negative size (n_triangles %lld, n_vertices %lld)", who, (long long)nt, (long long)nv);
+  if (nt > 0 && nv == 0 && nt <= max_triangles)
+    return fail(GSB_ERR_INVALID, "%s: %lld triangles but no vertices", who, (long long)nt);
+  return fail(GSB_ERR_INVALID, "%s: %lld triangles / %lld vertices; ids are 32-bit (at most %lld triangles and %lld vertices)",
+              who, (long long)nt, (long long)nv, (long long)max_triangles, (long long)kMaxMeshIds);
+}
+
 // ---------------------------------------------------------------------------------------------
 // Brick hash of the TSDF volume (Open3D's unordered_map<Vector3i, VolumeUnit>): open addressing, linear probing,
 // 64-bit keys = three 21-bit biased lattice indices.  An entry's position in the table identifies the brick inside a

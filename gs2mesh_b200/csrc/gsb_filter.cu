@@ -15,8 +15,7 @@
 namespace gsb {
 namespace {
 
-constexpr int64_t kMaxFilterIds = 2147483647;  // vertex ids are 32-bit, as in the other mesh entries
-constexpr double kWeightEps = 1e-12;           // Open3D's 1 / (|p_v - p_u| + 1e-12)
+constexpr double kWeightEps = 1e-12;  // Open3D's 1 / (|p_v - p_u| + 1e-12)
 
 enum FilterOp { kOpSimple = 0, kOpLaplacian = 1, kOpSharpen = 2 };
 
@@ -90,7 +89,7 @@ __global__ void __launch_bounds__(256) filter_pass_kernel(const long long* __res
   }
 }
 
-bool filter_sizes_ok(int64_t nv) { return nv >= 0 && nv <= kMaxFilterIds; }
+bool filter_sizes_ok(int64_t nv) { return nv >= 0 && nv <= kMaxMeshIds; }
 
 struct FilterWork {
   double* xyz[3];  // [3 nv] per attribute (position, colour, normal), NULL for an absent colour or normal
@@ -130,7 +129,7 @@ int gsb_mesh_filter(int kind, const double* vertices, const double* colors, cons
   if (iterations < 0) return fail(GSB_ERR_INVALID, "mesh_filter: iterations %d < 0", (int)iterations);
   if (!filter_sizes_ok(n_vertices))
     return fail(GSB_ERR_INVALID, "mesh_filter: %lld vertices; ids are 32-bit (at least 0 and at most %lld)",
-                (long long)n_vertices, (long long)kMaxFilterIds);
+                (long long)n_vertices, (long long)kMaxMeshIds);
   if ((!colors && out_colors) || (!normals && out_normals))
     return fail(GSB_ERR_INVALID, "mesh_filter: an output colour or normal array without its input");
   // neighbours may be NULL: a mesh without triangles has none, and only the offsets say so

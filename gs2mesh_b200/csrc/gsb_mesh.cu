@@ -318,9 +318,6 @@ __global__ void clean_sizes_kernel(const int* __restrict__ keep, const int* __re
   sizes[1] = nv ? (long long)new_id[nv - 1] + referenced[nv - 1] : 0;
 }
 
-// Ids are 32-bit inside the kernels; edge keys min*(n_vertices+1) + max then fit 62 bits.
-constexpr int64_t kMaxClusterIds = 2147483647;
-
 // Workspace layout of the two cluster entries (each carves its own regions from the start of the block); with a NULL
 // base only `total` is meaningful.
 struct ClusterWork {
@@ -382,17 +379,6 @@ CleanWork carve_clean(void* base, int64_t nt, int64_t nv) {
   return w;
 }
 
-bool cluster_sizes_ok(int64_t nt, int64_t nv) {
-  return nt >= 0 && nv >= 0 && nt <= kMaxClusterIds && nv <= kMaxClusterIds && (nt == 0 || nv > 0);
-}
-
-int cluster_size_error(const char* who, int64_t nt, int64_t nv) {
-  if (nt < 0 || nv < 0) return fail(GSB_ERR_INVALID, "%s: negative size (n_triangles %lld, n_vertices %lld)", who, (long long)nt, (long long)nv);
-  if (nt > 0 && nv == 0 && nt <= kMaxClusterIds) return fail(GSB_ERR_INVALID, "%s: %lld triangles but no vertices", who, (long long)nt);
-  return fail(GSB_ERR_INVALID, "%s: %lld triangles / %lld vertices; triangle and vertex ids are 32-bit (at most %lld each)", who,
-              (long long)nt, (long long)nv, (long long)kMaxClusterIds);
-}
-
 }  // namespace
 }  // namespace gsb
 
@@ -450,7 +436,7 @@ int gsb_mesh_vertex_normals(const double* xyz, int64_t n_vertices, const int64_t
 }
 
 size_t gsb_mesh_cluster_workspace_bytes(int64_t n_triangles, int64_t n_vertices) {
-  if (!cluster_sizes_ok(n_triangles, n_vertices)) return 0;
+  if (!mesh_sizes_ok(n_triangles, n_vertices, kMaxMeshIds)) return 0;
   const size_t a = carve_cluster(nullptr, n_triangles, n_vertices).total, b = carve_clean(nullptr, n_triangles, n_vertices).total;
   return a > b ? a : b;
 }
@@ -459,7 +445,8 @@ int gsb_mesh_clusters(const int64_t* triangles, int64_t n_triangles, int64_t n_v
                       size_t workspace_bytes, int64_t* labels, int64_t* counts, int64_t* n_clusters, double* cluster_area,
                       void* stream_v) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
-  if (!cluster_sizes_ok(n_triangles, n_vertices)) return cluster_size_error("mesh_clusters", n_triangles, n_vertices);
+  if (!mesh_sizes_ok(n_triangles, n_vertices, kMaxMeshIds))
+    return mesh_size_error("mesh_clusters", n_triangles, n_vertices, kMaxMeshIds);
   if (!n_clusters || (n_triangles && (!triangles || !workspace || !labels || !counts || (cluster_area && !vertices))))
     return fail(GSB_ERR_INVALID, "mesh_clusters: bad arguments");
   if (n_triangles == 0) {
@@ -473,7 +460,7 @@ int gsb_mesh_clusters(const int64_t* triangles, int64_t n_triangles, int64_t n_v
   const ClusterWork w = carve_cluster(workspace, n_triangles, n_vertices);
   const auto* tris = reinterpret_cast<const long long*>(triangles);
   const unsigned long long stride = (unsigned long long)n_vertices + 1;
-  const int key_bits = bits_of(stride * stride - 1);  // keys < (n_vertices+1)^2
+  const int key_bits = bits_of(stride * stride - 1);  // keys < (n_vertices+1)^2 <= 2^62: 32-bit ids
 
   cluster_edge_keys_kernel<<<blocks_for(nt), 256, 0, stream>>>(tris, nt, stride, w.keys, w.owner, w.parent);
   count_launch();
@@ -519,7 +506,8 @@ int gsb_mesh_remove_small_clusters(const int64_t* triangles, int64_t n_triangles
                                    const int64_t* counts, double threshold, void* workspace, size_t workspace_bytes,
                                    int64_t* out_triangles, int64_t* vertex_ids, int64_t* sizes, void* stream_v) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
-  if (!cluster_sizes_ok(n_triangles, n_vertices)) return cluster_size_error("mesh_remove_small_clusters", n_triangles, n_vertices);
+  if (!mesh_sizes_ok(n_triangles, n_vertices, kMaxMeshIds))
+    return mesh_size_error("mesh_remove_small_clusters", n_triangles, n_vertices, kMaxMeshIds);
   if (!sizes || (n_triangles && (!triangles || !labels || !counts || !out_triangles)) ||
       ((n_triangles || n_vertices) && !workspace) || (n_vertices && !vertex_ids))
     return fail(GSB_ERR_INVALID, "mesh_remove_small_clusters: bad arguments");

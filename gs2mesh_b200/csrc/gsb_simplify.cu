@@ -22,7 +22,6 @@
 namespace gsb {
 namespace {
 
-constexpr int64_t kMaxSimplifyIds = 2147483647;  // vertex, triangle and cell ids are 32-bit
 constexpr double kDetThreshold = 1e-4;            // Quadric::IsInvertible
 constexpr double kDblMin = 2.2250738585072014e-308;  // std::numeric_limits<double>::min(), LDLT's pivot tolerance
 
@@ -400,10 +399,6 @@ SimplifyWork carve_simplify(void* base, int64_t nv, int64_t nt) {
   return w;
 }
 
-bool simplify_sizes_ok(int64_t nv, int64_t nt) {
-  return nv >= 0 && nt >= 0 && nv <= kMaxSimplifyIds && nt <= kMaxSimplifyIds && (nt == 0 || nv > 0);
-}
-
 bool finite3(const double* v) { return std::isfinite(v[0]) && std::isfinite(v[1]) && std::isfinite(v[2]); }
 
 }  // namespace
@@ -414,7 +409,7 @@ using namespace gsb;
 extern "C" {
 
 size_t gsb_mesh_simplify_workspace_bytes(int64_t n_vertices, int64_t n_triangles) {
-  if (!simplify_sizes_ok(n_vertices, n_triangles)) return 0;
+  if (!mesh_sizes_ok(n_triangles, n_vertices, kMaxMeshIds)) return 0;
   return carve_simplify(nullptr, n_vertices, n_triangles).total;
 }
 
@@ -423,15 +418,8 @@ int gsb_mesh_simplify(const double* vertices, const double* colors, const double
                       double voxel_size, int contraction, void* workspace, size_t workspace_bytes, double* out_vertices,
                       double* out_colors, double* out_normals, int64_t* out_triangles, int64_t* sizes, void* stream_v) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
-  if (!simplify_sizes_ok(n_vertices, n_triangles)) {
-    if (n_vertices < 0 || n_triangles < 0)
-      return fail(GSB_ERR_INVALID, "mesh_simplify: negative size (n_vertices %lld, n_triangles %lld)", (long long)n_vertices,
-                  (long long)n_triangles);
-    if (n_triangles > 0 && n_vertices == 0 && n_triangles <= kMaxSimplifyIds)
-      return fail(GSB_ERR_INVALID, "mesh_simplify: %lld triangles but no vertices", (long long)n_triangles);
-    return fail(GSB_ERR_INVALID, "mesh_simplify: %lld vertices / %lld triangles; ids are 32-bit (at most %lld each)",
-                (long long)n_vertices, (long long)n_triangles, (long long)kMaxSimplifyIds);
-  }
+  if (!mesh_sizes_ok(n_triangles, n_vertices, kMaxMeshIds))
+    return mesh_size_error("mesh_simplify", n_triangles, n_vertices, kMaxMeshIds);
   if (contraction != GSB_SIMPLIFY_AVERAGE && contraction != GSB_SIMPLIFY_QUADRIC)
     return fail(GSB_ERR_INVALID, "mesh_simplify: unknown contraction %d", contraction);
   if (!sizes || !min_bound || !max_bound ||

@@ -235,71 +235,6 @@ size_t voxel_workspace_bytes(int64_t n_points) {
   return c.total();
 }
 
-// gsb_eval_voxel_downsample and gsb_pcd_voxel_downsample: keys, stable sort, voxel heads, their starts, then the mean of
-// the points and of the colours and normals that are given.  `who` prefixes the messages.
-int voxel_downsample(const char* who, const double* points, const double* colors, const double* normals, int64_t n_points,
-                     const double* min_bound, const double* max_bound, double voxel_size, void* workspace,
-                     size_t workspace_bytes, double* out, double* out_colors, double* out_normals, int64_t* n_out,
-                     cudaStream_t stream) {
-  if (n_points < 0 || n_points >= 2147483647 || !(voxel_size > 0.0) || !(voxel_size < INFINITY) || !min_bound || !max_bound ||
-      !n_out || (n_points && (!points || !out || !workspace)))
-    return fail(GSB_ERR_INVALID, "%s: bad arguments", who);
-  if (n_points == 0) {
-    GSB_CUDA_OK(cudaMemsetAsync(n_out, 0, sizeof(int64_t), stream));
-    return GSB_OK;
-  }
-  if (!host_finite(min_bound, 3) || !host_finite(max_bound, 3))
-    return fail(GSB_ERR_INVALID, "%s: the points are not finite", who);
-  VoxelGrid g;
-  g.voxel = voxel_size;
-  double span = 0.0;
-  for (int a = 0; a < 3; ++a) {
-    g.lo[a] = min_bound[a] - voxel_size * 0.5;
-    span = std::max(span, (max_bound[a] + voxel_size * 0.5) - g.lo[a]);
-  }
-  if (voxel_size * 2147483647.0 < span)  // Open3D: voxel_size * INT_MAX < (voxel_max_bound - voxel_min_bound).maxCoeff()
-    return fail(GSB_ERR_INVALID, "%s: voxel_size is too small (voxel_size * INT_MAX < %g)", who, span);
-  long long extent[3];  // voxels per axis; the largest index is that of max_bound
-  for (int a = 0; a < 3; ++a) extent[a] = (long long)std::floor((max_bound[a] - g.lo[a]) / voxel_size) + 1;
-  const int bx = bits_for(extent[0]), by = bits_for(extent[1]), bz = bits_for(extent[2]);
-  if (bx + by + bz > 63)
-    return fail(GSB_ERR_INVALID,
-                "%s: %lld x %lld x %lld voxels need %d key bits; voxel keys are limited to 63 bits", who,
-                extent[0], extent[1], extent[2], bx + by + bz);
-  g.shift_x = by + bz;
-  g.shift_y = bz;
-  if (workspace_bytes < voxel_workspace_bytes(n_points))
-    return fail(GSB_ERR_WORKSPACE, "%s: workspace %zu < %zu bytes", who, workspace_bytes,
-                voxel_workspace_bytes(n_points));
-  const int n = (int)n_points;
-  Carver c(workspace);
-  unsigned long long* keys = c.take<unsigned long long>(2 * (size_t)n);
-  long long* ids = c.take<long long>(3 * (size_t)n);
-  uint8_t* head = c.take<uint8_t>((size_t)n);
-  size_t tmp_bytes = workspace_bytes - c.total();
-  void* tmp = c.take<char>(tmp_bytes);
-  voxel_key_kernel<<<blocks_for(n), 256, 0, stream>>>(points, n, g, keys, ids);
-  count_launch();
-  GSB_CUDA_OK(cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, keys, keys + n, ids, ids + n, n, 0, bx + by + bz, stream));
-  voxel_head_kernel<<<blocks_for(n), 256, 0, stream>>>(keys + n, n, head);
-  count_launch();
-  long long* starts = ids + 2 * (size_t)n;
-  auto* n_voxels = reinterpret_cast<long long*>(n_out);
-  GSB_CUDA_OK(cub::DeviceSelect::Flagged(tmp, tmp_bytes, cub::CountingInputIterator<long long>(0), head, starts, n_voxels, n,
-                                         stream));
-  voxel_mean_kernel<<<blocks_for(n), 256, 0, stream>>>(points, n, ids + n, starts, n_voxels, false, out);
-  count_launch();
-  if (colors) {
-    voxel_mean_kernel<<<blocks_for(n), 256, 0, stream>>>(colors, n, ids + n, starts, n_voxels, false, out_colors);
-    count_launch();
-  }
-  if (normals) {
-    voxel_mean_kernel<<<blocks_for(n), 256, 0, stream>>>(normals, n, ids + n, starts, n_voxels, true, out_normals);
-    count_launch();
-  }
-  return check_launch("voxel downsample", stream, false);
-}
-
 }  // namespace
 }  // namespace gsb
 
@@ -346,22 +281,71 @@ int gsb_eval_crop_polygon(const double* points, int64_t n_points, const double* 
 
 size_t gsb_eval_voxel_workspace_bytes(int64_t n_points) { return voxel_workspace_bytes(n_points); }
 
-int gsb_eval_voxel_downsample(const double* points, int64_t n_points, const double* min_bound, const double* max_bound,
-                              double voxel_size, void* workspace, size_t workspace_bytes, double* out, int64_t* n_out,
-                              void* stream_v) {
-  return voxel_downsample("eval_voxel_downsample", points, nullptr, nullptr, n_points, min_bound, max_bound, voxel_size,
-                          workspace, workspace_bytes, out, nullptr, nullptr, n_out, static_cast<cudaStream_t>(stream_v));
-}
-
+// Keys, stable sort, voxel heads, their starts, then the mean of the points and of the colours and normals that are given.
 int gsb_pcd_voxel_downsample(const double* points, const double* colors, const double* normals, int64_t n_points,
                              const double* min_bound, const double* max_bound, double voxel_size, void* workspace,
                              size_t workspace_bytes, double* out, double* out_colors, double* out_normals, int64_t* n_out,
                              void* stream_v) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
   if (!colors != !out_colors || !normals != !out_normals)
     return fail(GSB_ERR_INVALID, "pcd_voxel_downsample: colours and normals need both their input and their output");
-  return voxel_downsample("pcd_voxel_downsample", points, colors, normals, n_points, min_bound, max_bound, voxel_size,
-                          workspace, workspace_bytes, out, out_colors, out_normals, n_out,
-                          static_cast<cudaStream_t>(stream_v));
+  if (n_points < 0 || n_points >= 2147483647 || !(voxel_size > 0.0) || !(voxel_size < INFINITY) || !min_bound || !max_bound ||
+      !n_out || (n_points && (!points || !out || !workspace)))
+    return fail(GSB_ERR_INVALID, "pcd_voxel_downsample: bad arguments");
+  if (n_points == 0) {
+    GSB_CUDA_OK(cudaMemsetAsync(n_out, 0, sizeof(int64_t), stream));
+    return GSB_OK;
+  }
+  if (!host_finite(min_bound, 3) || !host_finite(max_bound, 3))
+    return fail(GSB_ERR_INVALID, "pcd_voxel_downsample: the points are not finite");
+  VoxelGrid g;
+  g.voxel = voxel_size;
+  double span = 0.0;
+  for (int a = 0; a < 3; ++a) {
+    g.lo[a] = min_bound[a] - voxel_size * 0.5;
+    span = std::max(span, (max_bound[a] + voxel_size * 0.5) - g.lo[a]);
+  }
+  if (voxel_size * 2147483647.0 < span)  // Open3D: voxel_size * INT_MAX < (voxel_max_bound - voxel_min_bound).maxCoeff()
+    return fail(GSB_ERR_INVALID, "pcd_voxel_downsample: voxel_size is too small (voxel_size * INT_MAX < %g)", span);
+  long long extent[3];  // voxels per axis; the largest index is that of max_bound
+  for (int a = 0; a < 3; ++a) extent[a] = (long long)std::floor((max_bound[a] - g.lo[a]) / voxel_size) + 1;
+  const int bx = bits_for(extent[0]), by = bits_for(extent[1]), bz = bits_for(extent[2]);
+  if (bx + by + bz > 63)
+    return fail(GSB_ERR_INVALID,
+                "pcd_voxel_downsample: %lld x %lld x %lld voxels need %d key bits; voxel keys are limited to 63 bits",
+                extent[0], extent[1], extent[2], bx + by + bz);
+  g.shift_x = by + bz;
+  g.shift_y = bz;
+  if (workspace_bytes < voxel_workspace_bytes(n_points))
+    return fail(GSB_ERR_WORKSPACE, "pcd_voxel_downsample: workspace %zu < %zu bytes", workspace_bytes,
+                voxel_workspace_bytes(n_points));
+  const int n = (int)n_points;
+  Carver c(workspace);
+  unsigned long long* keys = c.take<unsigned long long>(2 * (size_t)n);
+  long long* ids = c.take<long long>(3 * (size_t)n);
+  uint8_t* head = c.take<uint8_t>((size_t)n);
+  size_t tmp_bytes = workspace_bytes - c.total();
+  void* tmp = c.take<char>(tmp_bytes);
+  voxel_key_kernel<<<blocks_for(n), 256, 0, stream>>>(points, n, g, keys, ids);
+  count_launch();
+  GSB_CUDA_OK(cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, keys, keys + n, ids, ids + n, n, 0, bx + by + bz, stream));
+  voxel_head_kernel<<<blocks_for(n), 256, 0, stream>>>(keys + n, n, head);
+  count_launch();
+  long long* starts = ids + 2 * (size_t)n;
+  auto* n_voxels = reinterpret_cast<long long*>(n_out);
+  GSB_CUDA_OK(cub::DeviceSelect::Flagged(tmp, tmp_bytes, cub::CountingInputIterator<long long>(0), head, starts, n_voxels, n,
+                                         stream));
+  voxel_mean_kernel<<<blocks_for(n), 256, 0, stream>>>(points, n, ids + n, starts, n_voxels, false, out);
+  count_launch();
+  if (colors) {
+    voxel_mean_kernel<<<blocks_for(n), 256, 0, stream>>>(colors, n, ids + n, starts, n_voxels, false, out_colors);
+    count_launch();
+  }
+  if (normals) {
+    voxel_mean_kernel<<<blocks_for(n), 256, 0, stream>>>(normals, n, ids + n, starts, n_voxels, true, out_normals);
+    count_launch();
+  }
+  return check_launch("voxel downsample", stream, false);
 }
 
 int gsb_eval_icp_moments(const double* source, const int64_t* index, const double* dist2, int64_t n_source,

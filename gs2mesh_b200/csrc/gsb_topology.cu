@@ -24,22 +24,10 @@ namespace {
 
 // 6 n_triangles link-graph slots (two nodes per (triangle, corner)) are int ids: n_triangles <= (2^31 - 1) / 6.
 constexpr int64_t kMaxTopoTriangles = 357913941;
-constexpr int64_t kMaxTopoVertices = 2147483647;
 constexpr int kLevels = 22;         // grid levels: 2^(20-L) + 1 cells per axis, L = 0 .. 21 (one cell)
 constexpr int kRegsPerTriangle = 4;  // the chosen level registers at most 4 n_triangles (triangle, cell) pairs
 constexpr int kNarrowBlocks = 132 * 8;  // grid-stride over the candidates: 8 blocks per SM of an H100 SXM
 constexpr double kEps = 1e-6;        // Moeller's EPSILON with USE_EPSILON_TEST
-
-bool topo_sizes_ok(int64_t nt, int64_t nv) {
-  return nt >= 0 && nv >= 0 && nt <= kMaxTopoTriangles && nv <= kMaxTopoVertices && (nt == 0 || nv > 0);
-}
-
-int topo_size_error(const char* who, int64_t nt, int64_t nv) {
-  if (nt < 0 || nv < 0) return fail(GSB_ERR_INVALID, "%s: negative size (n_triangles %lld, n_vertices %lld)", who, (long long)nt, (long long)nv);
-  if (nt > 0 && nv == 0 && nt <= kMaxTopoTriangles) return fail(GSB_ERR_INVALID, "%s: %lld triangles but no vertices", who, (long long)nt);
-  return fail(GSB_ERR_INVALID, "%s: %lld triangles / %lld vertices; ids are 32-bit (at most %lld triangles and %lld vertices)", who,
-              (long long)nt, (long long)nv, (long long)kMaxTopoTriangles, (long long)kMaxTopoVertices);
-}
 
 template <typename T>
 __device__ __forceinline__ long long upper_bound(const T* a, long long n, T x) {  // first index with a[i] > x
@@ -799,14 +787,15 @@ using namespace gsb;
 extern "C" {
 
 size_t gsb_mesh_edge_topology_workspace_bytes(int64_t n_triangles, int64_t n_vertices) {
-  if (!topo_sizes_ok(n_triangles, n_vertices)) return 0;
+  if (!mesh_sizes_ok(n_triangles, n_vertices, kMaxTopoTriangles)) return 0;
   return carve_edges(nullptr, n_triangles).total;
 }
 
 int gsb_mesh_edge_topology(const int64_t* triangles, int64_t n_triangles, int64_t n_vertices, int allow_boundary_edges,
                            void* workspace, size_t workspace_bytes, int64_t* out_edges, int64_t* sizes, void* stream_v) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
-  if (!topo_sizes_ok(n_triangles, n_vertices)) return topo_size_error("mesh_edge_topology", n_triangles, n_vertices);
+  if (!mesh_sizes_ok(n_triangles, n_vertices, kMaxTopoTriangles))
+    return mesh_size_error("mesh_edge_topology", n_triangles, n_vertices, kMaxTopoTriangles);
   if (!sizes || (n_triangles && (!triangles || !workspace))) return fail(GSB_ERR_INVALID, "mesh_edge_topology: bad arguments");
   const size_t need = gsb_mesh_edge_topology_workspace_bytes(n_triangles, n_vertices);
   if (n_triangles && workspace_bytes < need)
@@ -855,14 +844,15 @@ int gsb_mesh_edge_topology(const int64_t* triangles, int64_t n_triangles, int64_
 }
 
 size_t gsb_mesh_vertex_topology_workspace_bytes(int64_t n_triangles, int64_t n_vertices) {
-  if (!topo_sizes_ok(n_triangles, n_vertices)) return 0;
+  if (!mesh_sizes_ok(n_triangles, n_vertices, kMaxTopoTriangles)) return 0;
   return carve_vertices(nullptr, n_triangles, n_vertices).total;
 }
 
 int gsb_mesh_non_manifold_vertices(const int64_t* triangles, int64_t n_triangles, int64_t n_vertices, void* workspace,
                                    size_t workspace_bytes, int64_t* out_vertices, int64_t* count, void* stream_v) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
-  if (!topo_sizes_ok(n_triangles, n_vertices)) return topo_size_error("mesh_non_manifold_vertices", n_triangles, n_vertices);
+  if (!mesh_sizes_ok(n_triangles, n_vertices, kMaxTopoTriangles))
+    return mesh_size_error("mesh_non_manifold_vertices", n_triangles, n_vertices, kMaxTopoTriangles);
   if (!count || (n_triangles && (!triangles || !workspace)))
     return fail(GSB_ERR_INVALID, "mesh_non_manifold_vertices: bad arguments");
   const size_t need = gsb_mesh_vertex_topology_workspace_bytes(n_triangles, n_vertices);
@@ -908,7 +898,8 @@ int gsb_mesh_non_manifold_vertices(const int64_t* triangles, int64_t n_triangles
 }
 
 size_t gsb_mesh_self_intersections_workspace_bytes(int64_t n_triangles, int64_t n_vertices, int64_t capacity) {
-  if (!topo_sizes_ok(n_triangles, n_vertices) || capacity < 0 || capacity > n_triangles * (n_triangles - 1) / 2) return 0;
+  if (!mesh_sizes_ok(n_triangles, n_vertices, kMaxTopoTriangles) || capacity < 0 || capacity > n_triangles * (n_triangles - 1) / 2)
+    return 0;
   return carve_isect(nullptr, n_triangles, capacity).total_bytes;
 }
 
@@ -917,7 +908,8 @@ int gsb_mesh_self_intersections(const double* vertices, int64_t n_vertices, cons
                                 int64_t* out_pairs, int64_t capacity, int64_t* stats, void* stream_v) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
   const char* who = "mesh_self_intersections";
-  if (!topo_sizes_ok(n_triangles, n_vertices)) return topo_size_error(who, n_triangles, n_vertices);
+  if (!mesh_sizes_ok(n_triangles, n_vertices, kMaxTopoTriangles))
+    return mesh_size_error(who, n_triangles, n_vertices, kMaxTopoTriangles);
   if (capacity < 0 || capacity > n_triangles * (n_triangles - 1) / 2)
     return fail(GSB_ERR_INVALID, "%s: capacity %lld outside [0, n_triangles (n_triangles - 1) / 2]", who, (long long)capacity);
   if (!stats || (n_triangles && (!vertices || !triangles || !workspace || !min_bound || !max_bound)) || (capacity && !out_pairs))
@@ -994,14 +986,15 @@ int gsb_mesh_self_intersections(const double* vertices, int64_t n_vertices, cons
 }
 
 size_t gsb_mesh_area_volume_workspace_bytes(int64_t n_triangles, int64_t n_vertices) {
-  if (!topo_sizes_ok(n_triangles, n_vertices)) return 0;
+  if (!mesh_sizes_ok(n_triangles, n_vertices, kMaxTopoTriangles)) return 0;
   return area_volume_bytes(n_triangles);
 }
 
 int gsb_mesh_area_volume(const double* vertices, int64_t n_vertices, const int64_t* triangles, int64_t n_triangles,
                          void* workspace, size_t workspace_bytes, double* out, void* stream_v) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
-  if (!topo_sizes_ok(n_triangles, n_vertices)) return topo_size_error("mesh_area_volume", n_triangles, n_vertices);
+  if (!mesh_sizes_ok(n_triangles, n_vertices, kMaxTopoTriangles))
+    return mesh_size_error("mesh_area_volume", n_triangles, n_vertices, kMaxTopoTriangles);
   if (!out || (n_triangles && (!vertices || !triangles || !workspace))) return fail(GSB_ERR_INVALID, "mesh_area_volume: bad arguments");
   const size_t need = gsb_mesh_area_volume_workspace_bytes(n_triangles, n_vertices);
   if (n_triangles && workspace_bytes < need)

@@ -233,13 +233,28 @@ def read_triangle_mesh_ply(path, with_colors=False):
     return xyz, tris, colors
 
 
-def write_point_cloud_ply(path, points, colors=None, normals=None):
-    """o3d.io.write_point_cloud for eval.py's visualisation clouds (eval.py:21-25): binary little-endian, double xyz,
-    double normals nx ny nz when given, uchar rgb = round(255 * colour), in Open3D's property order."""
+def color_to_uint8(colors):
+    """Open3D's utility::ColorToUint8, which its PLY writer applies to colours:
+    uint8_t(std::round(std::min(1., std::max(0., c)) * 255.)).  std::round rounds halves away from zero (np.rint would
+    round them to even), and std::max(0., NaN) is 0."""
+    c = np.asarray(colors, dtype=np.float64)
+    c = np.where(c > 0.0, c, 0.0)
+    s = np.where(c < 1.0, c, 1.0) * 255.0
+    lo = np.floor(s)
+    return (lo + (s - lo >= 0.5)).astype(np.uint8)
+
+
+def write_point_cloud_ply(path, points, colors=None, normals=None, triangles=None):
+    """o3d.io.write_point_cloud (eval.py's visualisation clouds, eval.py:21-25), and with `triangles`
+    o3d.io.write_triangle_mesh: binary little-endian, double xyz, double normals nx ny nz when given, uchar rgb =
+    color_to_uint8(colour) when given, in Open3D's property order.  A mesh file also carries a `comment Created by
+    gs2mesh_b200` header line and, after the vertices, a face element of uchar-counted uint triangles."""
     points = np.asarray(points, dtype=np.float64).reshape(-1, 3)
     props = [("x", "<f8"), ("y", "<f8"), ("z", "<f8")]
-    header = ["ply", "format binary_little_endian 1.0", f"element vertex {len(points)}", "property double x",
-              "property double y", "property double z"]
+    header = ["ply", "format binary_little_endian 1.0"]
+    if triangles is not None:
+        header.append("comment Created by gs2mesh_b200")
+    header += [f"element vertex {len(points)}", "property double x", "property double y", "property double z"]
     if normals is not None:
         props += [("nx", "<f8"), ("ny", "<f8"), ("nz", "<f8")]
         header += ["property double nx", "property double ny", "property double nz"]
@@ -251,11 +266,17 @@ def write_point_cloud_ply(path, points, colors=None, normals=None):
     if normals is not None:
         tab["nx"], tab["ny"], tab["nz"] = np.asarray(normals, dtype=np.float64).reshape(-1, 3).T
     if colors is not None:
-        rgb = np.clip(np.rint(np.asarray(colors, dtype=np.float64).reshape(-1, 3) * 255.0), 0, 255).astype(np.uint8)
-        tab["red"], tab["green"], tab["blue"] = rgb.T
+        tab["red"], tab["green"], tab["blue"] = color_to_uint8(colors).reshape(-1, 3).T
+    face = np.zeros(0, dtype=[("n", "u1"), ("v", "<u4", (3,))])
+    if triangles is not None:
+        tris = np.asarray(triangles).reshape(-1, 3)
+        face = np.zeros(len(tris), dtype=face.dtype)
+        face["n"], face["v"] = 3, tris.astype(np.uint32)
+        header += [f"element face {len(face)}", "property list uchar uint vertex_indices"]
     with open(path, "wb") as f:
         f.write(("\n".join(header + ["end_header"]) + "\n").encode("ascii"))
         f.write(tab.tobytes())
+        f.write(face.tobytes())
     return path
 
 

@@ -26,17 +26,7 @@ import torch
 from . import _lib
 from . import pointcloud as _pcd
 from ._lib import ptr
-
-
-def color_to_uint8(colors):
-    """Open3D's utility::ColorToUint8, which its PLY writer applies to vertex colours:
-    uint8_t(std::round(std::min(1., std::max(0., c)) * 255.)).  std::round rounds halves away from zero (np.rint would
-    round them to even), and std::max(0., NaN) is 0."""
-    c = np.asarray(colors, dtype=np.float64)
-    c = np.where(c > 0.0, c, 0.0)
-    s = np.where(c < 1.0, c, 1.0) * 255.0
-    lo = np.floor(s)
-    return (lo + (s - lo >= 0.5)).astype(np.uint8)
+from .io import color_to_uint8, write_point_cloud_ply  # noqa: F401  (color_to_uint8: callers also import it from here)
 
 
 class SimplificationContraction(enum.IntEnum):
@@ -79,6 +69,18 @@ class TriangleMesh:
         self.vertex_colors = None if vertex_colors is None else np.asarray(vertex_colors, dtype=np.float64).reshape(-1, 3)
         self.vertex_normals = None if vertex_normals is None else np.asarray(vertex_normals, dtype=np.float64).reshape(-1, 3)
 
+    def _check(self, who, attributes=False):
+        """(n_vertices, n_triangles); ValueError prefixed `who: ` for a triangle index outside [0, n_vertices) and, with
+        `attributes`, for vertex colours or normals without one row per vertex."""
+        nv, nt = len(self.vertices), len(self.triangles)
+        if nt and (self.triangles.min() < 0 or self.triangles.max() >= nv):
+            raise ValueError(f"{who}: triangle vertex index out of range")
+        for name in ("vertex_colors", "vertex_normals") if attributes else ():
+            a = getattr(self, name)
+            if a is not None and len(a) != nv:
+                raise ValueError(f"{who}: {name} must have one row per vertex")
+        return nv, nt
+
     # -- tsdf_utils.py:109
     def scale(self, scale, center=(0, 0, 0)):
         c = np.asarray(center, dtype=np.float64)
@@ -91,8 +93,7 @@ class TriangleMesh:
         if nv == 0:
             self.vertex_normals = np.zeros((0, 3))
             return self
-        if nt and (self.triangles.min() < 0 or self.triangles.max() >= nv):
-            raise ValueError("compute_vertex_normals: triangle vertex index out of range")
+        self._check("compute_vertex_normals")
         dev = _lib.device(device)
         with torch.cuda.device(dev):
             xyz = torch.as_tensor(self.vertices).to(dev).contiguous()
@@ -113,9 +114,7 @@ class TriangleMesh:
     def _clusters_on_device(self, with_area):
         """gsb_mesh_clusters on self.device: (device triangles, workspace, labels, counts, n_clusters, cluster areas or
         None), all enqueued on the device's current stream."""
-        nv, nt = len(self.vertices), len(self.triangles)
-        if nt and (self.triangles.min() < 0 or self.triangles.max() >= nv):
-            raise ValueError("cluster_connected_triangles: triangle vertex index out of range")
+        nv, nt = self._check("cluster_connected_triangles")
         dev = self.device
         L = _lib.lib()
         stream = _lib.stream(dev)
@@ -208,13 +207,7 @@ class TriangleMesh:
         s = float(voxel_size)
         if not s > 0.0:
             raise RuntimeError("voxel_size <= 0.0")
-        nv, nt = len(self.vertices), len(self.triangles)
-        if nt and (self.triangles.min() < 0 or self.triangles.max() >= nv):
-            raise ValueError("simplify_vertex_clustering: triangle vertex index out of range")
-        for name in ("vertex_colors", "vertex_normals"):
-            a = getattr(self, name)
-            if a is not None and len(a) != nv:
-                raise ValueError(f"simplify_vertex_clustering: {name} must have one row per vertex")
+        nv, nt = self._check("simplify_vertex_clustering", attributes=True)
         lo = self.vertices.min(axis=0) if nv else np.zeros(3)
         hi = self.vertices.max(axis=0) if nv else np.zeros(3)
         dev = _lib.device(self.device)
@@ -270,13 +263,7 @@ class TriangleMesh:
         iterations = int(number_of_iterations)
         if not 0 <= iterations <= 2**31 - 1:
             raise ValueError(f"{name}: number_of_iterations must be in [0, 2^31 - 1], got {iterations}")
-        nv, nt = len(self.vertices), len(self.triangles)
-        if nt and (self.triangles.min() < 0 or self.triangles.max() >= nv):
-            raise ValueError(f"{name}: triangle vertex index out of range")
-        for attr in ("vertex_colors", "vertex_normals"):
-            a = getattr(self, attr)
-            if a is not None and len(a) != nv:
-                raise ValueError(f"{name}: {attr} must have one row per vertex")
+        nv, nt = self._check(name, attributes=True)
         dev = _lib.device(self.device)
         L = _lib.lib()
         with torch.cuda.device(dev):
@@ -356,33 +343,9 @@ class TriangleMesh:
                 raise RuntimeError("The mesh is not orientable, and the volume cannot be computed.")
             return abs(q.area_volume()[1])
 
-    # -- o3d.io.write_triangle_mesh(path, mesh): binary little-endian PLY, double coordinates
+    # -- o3d.io.write_triangle_mesh(path, mesh): binary little-endian PLY, double coordinates and normals, uchar colours
     def write_ply(self, path):
-        nv, nt = len(self.vertices), len(self.triangles)
-        props = [("x", "<f8"), ("y", "<f8"), ("z", "<f8")]
-        header = ["ply", "format binary_little_endian 1.0", "comment Created by gs2mesh_b200", f"element vertex {nv}",
-                  "property double x", "property double y", "property double z"]
-        if self.vertex_normals is not None:
-            props += [("nx", "<f8"), ("ny", "<f8"), ("nz", "<f8")]
-            header += ["property double nx", "property double ny", "property double nz"]
-        if self.vertex_colors is not None:
-            props += [("red", "u1"), ("green", "u1"), ("blue", "u1")]
-            header += ["property uchar red", "property uchar green", "property uchar blue"]
-        header += [f"element face {nt}", "property list uchar uint vertex_indices", "end_header"]
-        vert = np.zeros(nv, dtype=props)
-        vert["x"], vert["y"], vert["z"] = self.vertices.T if nv else (np.zeros(0),) * 3
-        if self.vertex_normals is not None and nv:
-            vert["nx"], vert["ny"], vert["nz"] = self.vertex_normals.T
-        if self.vertex_colors is not None and nv:
-            vert["red"], vert["green"], vert["blue"] = color_to_uint8(self.vertex_colors).T
-        face = np.zeros(nt, dtype=[("n", "u1"), ("v", "<u4", (3,))])
-        face["n"] = 3
-        face["v"] = self.triangles.astype(np.uint32)
-        with open(path, "wb") as f:
-            f.write(("\n".join(header) + "\n").encode("ascii"))
-            f.write(vert.tobytes())
-            f.write(face.tobytes())
-        return path
+        return write_point_cloud_ply(path, self.vertices, self.vertex_colors, self.vertex_normals, self.triangles)
 
 
 class _Topology:
@@ -390,9 +353,7 @@ class _Topology:
     so that is_watertight and get_volume run it once."""
 
     def __init__(self, mesh):
-        nv, nt = len(mesh.vertices), len(mesh.triangles)
-        if nt and (mesh.triangles.min() < 0 or mesh.triangles.max() >= nv):
-            raise ValueError("topology: triangle vertex index out of range")
+        nv, nt = mesh._check("topology")
         if not np.isfinite(mesh.vertices).all():
             raise ValueError("topology: the vertices are not finite")
         self.mesh, self.nv, self.nt = mesh, nv, nt
@@ -608,8 +569,6 @@ class PointCloud:
 
     # -- o3d.io.write_point_cloud(path, pcd): binary little-endian PLY, double coordinates and normals, uchar colours
     def write_ply(self, path):
-        from .io import write_point_cloud_ply
-
         return write_point_cloud_ply(path, self.points, self.colors, self.normals)
 
 

@@ -22,7 +22,7 @@ import torch
 from . import _lib
 from ._lib import ptr
 from .evaluate import PointGrid
-from .tnt import compute_point_cloud_distance as _cloud_distance
+from .tnt import _voxel_downsample, compute_point_cloud_distance as _cloud_distance
 
 MAX_POINTS = 2**31 - 1
 
@@ -187,23 +187,14 @@ def voxel_down_sample(pcd, voxel_size):
     if n == 0:
         return _empty_like(pcd)
     dev = _lib.device(pcd.device)
-    L = _lib.lib()
-    dbl3 = C.c_double * 3
     with torch.cuda.device(dev):
-        xyz, rgb, nrm = _upload(pcd, dev)
-        like = lambda t: None if t is None else torch.empty_like(t)
-        out, out_c, out_n = like(xyz), like(rgb), like(nrm)
-        work = torch.empty(int(L.gsb_eval_voxel_workspace_bytes(n)), dtype=torch.uint8, device=dev)
-        count = torch.empty(1, dtype=torch.int64, device=dev)
-        rc = L.gsb_pcd_voxel_downsample(ptr(xyz), ptr(rgb), ptr(nrm), n, dbl3(*pcd.points.min(axis=0).tolist()),
-                                        dbl3(*pcd.points.max(axis=0).tolist()), s, ptr(work), work.numel(), ptr(out),
-                                        ptr(out_c), ptr(out_n), ptr(count), _lib.stream(dev))
-        if rc == _lib.GSB_ERR_INVALID and b"voxel_size is too small" in L.gsb_last_error():
-            raise RuntimeError("voxel_size is too small.")
-        _lib.check(rc, invalid_is_value_error=True)
-        m = int(count.item())
-        head = lambda t: None if t is None else t[:m]
-        return _new(pcd, dev, head(out), head(out_c), head(out_n))
+        try:
+            out = _voxel_downsample(*_upload(pcd, dev), s)
+        except ValueError as e:
+            if "voxel_size is too small" in str(e):
+                raise RuntimeError("voxel_size is too small.") from None
+            raise
+        return _new(pcd, dev, *out)
 
 
 def compute_nearest_neighbor_distance(pcd):

@@ -9,8 +9,8 @@ Restated (file:line under evaluation/TNT/eval_code/python_toolbox/evaluation):
   plot.py:40-109           plot_graph (only when matplotlib is installed)
 
 The Open3D 0.17 operations underneath (PointCloud.Transform, CropInPolygon, VoxelDownSample, RegistrationICP with
-TransformationEstimationPointToPoint, EstimateNormals) are gsb_eval_* kernels of include/gs2mesh_b200.h
-(gs2mesh_b200/csrc/gsb_tnt.cu, gsb_eval.cu, gsb_normals.cu); DESIGN.md section 7d gives their operation orders.  Host work per ICP iteration is the 3x3 SVD and two
+TransformationEstimationPointToPoint, EstimateNormals) are gsb_eval_* kernels of include/gs2mesh_b200.h, and
+gsb_pcd_voxel_downsample for VoxelDownSample (gs2mesh_b200/csrc/gsb_tnt.cu, gsb_eval.cu, gsb_normals.cu); DESIGN.md section 7d gives their operation orders.  Host work per ICP iteration is the 3x3 SVD and two
 reads of 13 moments.  There is no CPU fallback.  The rough RANSAC alignment runs on the host over the camera centres
 with a seeded generator: it is the one step that cannot equal Open3D's bits (its random sequence is not reproducible).
 """
@@ -139,24 +139,32 @@ def voxel_down_sample(points, voxel_size):
     """PointCloud.voxel_down_sample: the mean of each voxel's points (summed in input order).  Open3D emits the voxels
     in hash-map order; here they come in ascending (x, y, z) voxel order, the same set of points."""
     p = _points(points)
-    dev = p.device
-    n = p.shape[0]
     if not float(voxel_size) > 0.0:
         raise ValueError("voxel_down_sample: voxel_size <= 0")
-    if n == 0:
+    if p.shape[0] == 0:
         return p.clone()
-    lo = p.min(dim=0).values.cpu().numpy()
-    hi = p.max(dim=0).values.cpu().numpy()
+    return _voxel_downsample(p, None, None, float(voxel_size))[0]
+
+
+def _voxel_downsample(xyz, rgb, nrm, voxel_size):
+    """gsb_pcd_voxel_downsample of a non-empty cloud: device fp64 [n,3] points, colours or None and normals or None ->
+    (points, colours, normals) of the voxels, None where none was given.  The library's refusals are ValueErrors."""
+    dev = xyz.device
+    n = xyz.shape[0]
     L = _lib.lib()
-    ws = torch.empty(int(L.gsb_eval_voxel_workspace_bytes(n)), dtype=torch.uint8, device=dev)
-    out = torch.empty_like(p)
-    count = torch.empty(1, dtype=torch.int64, device=dev)
     dbl3 = C.c_double * 3
     with torch.cuda.device(dev):
-        rc = L.gsb_eval_voxel_downsample(ptr(p), n, dbl3(*lo.tolist()), dbl3(*hi.tolist()), float(voxel_size), ptr(ws),
-                                         ws.numel(), ptr(out), ptr(count), _lib.stream(dev))
-    _lib.check(rc, invalid_is_value_error=True)
-    return out[:int(count.item())]
+        like = lambda t: None if t is None else torch.empty_like(t)
+        out, out_c, out_n = like(xyz), like(rgb), like(nrm)
+        ws = torch.empty(int(L.gsb_eval_voxel_workspace_bytes(n)), dtype=torch.uint8, device=dev)
+        count = torch.empty(1, dtype=torch.int64, device=dev)
+        rc = L.gsb_pcd_voxel_downsample(ptr(xyz), ptr(rgb), ptr(nrm), n, dbl3(*xyz.min(dim=0).values.tolist()),
+                                        dbl3(*xyz.max(dim=0).values.tolist()), voxel_size, ptr(ws), ws.numel(), ptr(out),
+                                        ptr(out_c), ptr(out_n), ptr(count), _lib.stream(dev))
+        _lib.check(rc, invalid_is_value_error=True)
+        m = int(count.item())
+    head = lambda t: None if t is None else t[:m]
+    return head(out), head(out_c), head(out_n)
 
 
 def uniform_down_sample(points, every_k_points):
@@ -474,11 +482,9 @@ def write_color_distances(path, points, distances, max_distance, normals=None):
     if plt is None:
         return None
     from .io import write_point_cloud_ply
-    from .mesh import color_to_uint8
 
     colors = plt.get_cmap("hot_r")(np.minimum(np.asarray(distances), max_distance) / max_distance)[:, :3]
-    # write_point_cloud_ply rounds colour*255 with np.rint; pass colours already on Open3D's uint8 grid
-    return write_point_cloud_ply(path, points, color_to_uint8(colors) / 255.0, normals)
+    return write_point_cloud_ply(path, points, colors, normals)
 
 
 def plot_graph(scene, fscore, dist_threshold, edges_source, cum_source, edges_target, cum_target, plot_stretch,

@@ -608,12 +608,6 @@ int gsb_pcd_radius_outliers(const GsbPointGrid* grid, int64_t nb_points, double 
  *                              polygon: device double [n_vertices,3], 3 <= n_vertices <= GSB_EVAL_MAX_POLYGON.
  *                              counter: device uint32 scratch; host_non_finite: pinned host uint32.  SYNCHRONISES the
  *                              stream and returns GSB_ERR_INVALID when a point is not finite.
- *   gsb_eval_voxel_downsample  the mean of the points of each voxel floor((p - lo) / voxel_size), lo = min_bound -
- *                              voxel_size/2, summed in input order, one output point per voxel in ascending (x, y, z)
- *                              voxel order.  min_bound / max_bound: host double [3], the points' bounds.  out: device
- *                              double [n_points,3]; n_out: device int64, the number of voxels.  GSB_ERR_INVALID when
- *                              voxel_size * INT_MAX < the padded extent (Open3D's "voxel_size is too small") or when the
- *                              voxel keys need more than 63 bits.  n_points < 2^31.
  *   gsb_eval_icp_correspond    index[i] = the nearest grid point with ((dx*dx)+dy*dy)+dz*dz < radius*radius, else -1;
  *                              dist2[i] its squared distance (+inf for -1).  A source point with a NaN or infinite
  *                              coordinate gets -1.
@@ -629,16 +623,17 @@ int gsb_eval_transform_points(const double* points, int64_t n_points, const doub
 int gsb_eval_crop_polygon(const double* points, int64_t n_points, const double* polygon, int32_t n_vertices,
                           int32_t orthogonal_axis, double axis_min, double axis_max, uint8_t* keep, uint32_t* counter,
                           uint32_t* host_non_finite, void* stream);
+/* PointCloud::VoxelDownSample, with colours and normals (DESIGN.md sections 7d and 7, "Point-cloud cleaning and
+ * downsampling"): the mean of the points of each voxel floor((p - lo) / voxel_size), lo = min_bound - voxel_size/2,
+ * summed in input order, one output point per voxel in ascending (x, y, z) voxel order.  min_bound / max_bound: host
+ * double [3], the points' bounds.  out: device double [n_points,3]; n_out: device int64, the number of voxels.
+ * colors / normals: device double [n_points,3] or NULL, each given together with its output out_colors / out_normals
+ * (device double [n_points,3]).  Each voxel's colour and normal is the sum over its points in input order from 0.0,
+ * divided by double(the voxel's point count); a normal with a NaN component adds nothing but its point still counts
+ * (Open3D's AccumulatedPoint).  Normals are not renormalised.  GSB_ERR_INVALID when voxel_size * INT_MAX < the padded
+ * extent (Open3D's "voxel_size is too small") or when the voxel keys need more than 63 bits.  n_points < 2^31.
+ * workspace: gsb_eval_voxel_workspace_bytes(n_points) bytes (0 for invalid sizes), else GSB_ERR_WORKSPACE. */
 size_t gsb_eval_voxel_workspace_bytes(int64_t n_points);
-int gsb_eval_voxel_downsample(const double* points, int64_t n_points, const double* min_bound, const double* max_bound,
-                              double voxel_size, void* workspace, size_t workspace_bytes, double* out, int64_t* n_out,
-                              void* stream);
-/* PointCloud::VoxelDownSample with colours and normals (DESIGN.md section 7, "Point-cloud cleaning and downsampling"):
- * gsb_eval_voxel_downsample's voxels, order, points and refusals, with the same workspace
- * (gsb_eval_voxel_workspace_bytes).  colors / normals: device double [n_points,3] or NULL, each given together with its
- * output out_colors / out_normals (device double [n_points,3]), else GSB_ERR_INVALID.  Each voxel's colour and normal is
- * the sum over its points in input order from 0.0, divided by double(the voxel's point count); a normal with a NaN
- * component adds nothing but its point still counts (Open3D's AccumulatedPoint).  Normals are not renormalised. */
 int gsb_pcd_voxel_downsample(const double* points, const double* colors, const double* normals, int64_t n_points,
                              const double* min_bound, const double* max_bound, double voxel_size, void* workspace,
                              size_t workspace_bytes, double* out, double* out_colors, double* out_normals, int64_t* n_out,

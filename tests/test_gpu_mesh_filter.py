@@ -224,7 +224,7 @@ def test_o3d_compat_call_sequence_and_ply_round_trip(gsb_lib, cuda_device, tmp_p
 
     import gs2mesh_b200.o3d_compat as o3d
     from gs2mesh_b200.io import read_triangle_mesh_ply
-    from gs2mesh_b200.mesh import color_to_uint8
+    from gs2mesh_b200.io import color_to_uint8
     from tests.test_gpu_tsdf import CX, CY, FX, FY, TRUNC, VL, W, H, _views
 
     with torch.cuda.device(cuda_device):

@@ -215,6 +215,6 @@ def test_o3d_compat_call_sequence_and_ply_round_trip(gsb_lib, cuda_device, tmp_p
         assert o3d.io.write_triangle_mesh(path, small)
         xyz, tris, rgb = read_triangle_mesh_ply(path, with_colors=True)
         assert xyz.tobytes() == small.vertices.tobytes() and (tris == small.triangles).all()
-        from gs2mesh_b200.mesh import color_to_uint8
+        from gs2mesh_b200.io import color_to_uint8
 
         assert (rgb == color_to_uint8(small.vertex_colors) / 255.0).all()

@@ -14,8 +14,10 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 def test_write_ply_rounds_colour_halves_away_from_zero(tmp_path):
     """Open3D's PLY writer stores utility::ColorToUint8(c) = uint8(std::round(min(1, max(0, c)) * 255)): clamp first, then
-    round half away from zero.  np.rint would round the exact halves to even."""
-    from gs2mesh_b200.mesh import TriangleMesh, color_to_uint8
+    round half away from zero.  np.rint would round the exact halves to even.  Meshes and point clouds write the same
+    vertex records."""
+    from gs2mesh_b200.io import color_to_uint8, write_point_cloud_ply
+    from gs2mesh_b200.mesh import PointCloud, TriangleMesh
 
     halves = np.array([(k + 0.5) / 255.0 for k in range(255)])
     halves = halves[halves * 255.0 == np.arange(255)[: len(halves)] + 0.5]  # products that are exactly k + 0.5
@@ -40,6 +42,8 @@ def test_write_ply_rounds_colour_halves_away_from_zero(tmp_path):
     rec = np.frombuffer(body, dtype=[("xyz", "<f8", (3,)), ("rgb", "u1", (3,))])
     np.testing.assert_array_equal(rec["xyz"], v)
     np.testing.assert_array_equal(rec["rgb"], want)
+    for cloud in (PointCloud(v, c).write_ply(str(tmp_path / "p.ply")), write_point_cloud_ply(str(tmp_path / "q.ply"), v, c)):
+        assert open(cloud, "rb").read().split(b"end_header\n")[1] == body
 
 
 def _clean_by_union_find(v, t, colors, threshold):

@@ -272,6 +272,3 @@ def test_c_entry_points_refuse_bad_arguments(gsb_lib):
     assert call(fake, fake, fake, 10, lo, huge, 1.0, fake, vws, fake, fake, fake, fake) == _lib.GSB_ERR_INVALID
     assert b"63 bits" in L.gsb_last_error()
     assert call(fake, fake, fake, 10, lo, hi, 0.1, fake, vws - 1, fake, fake, fake, fake) == _lib.GSB_ERR_WORKSPACE
-    # the points-only entry keeps its own messages
-    assert L.gsb_eval_voxel_downsample(fake, 10, lo, far, 1e-7, fake, vws, fake, fake, None) == _lib.GSB_ERR_INVALID
-    assert L.gsb_last_error().startswith(b"eval_voxel_downsample: voxel_size is too small")

@@ -318,20 +318,8 @@ def test_c_entry_points_refuse_bad_arguments(gsb_lib):
         assert L.gsb_eval_crop_polygon(fake, 10, fake, nv, axis, 0.0, 1.0, fake, fake, fake, None) == _lib.GSB_ERR_INVALID
     assert b"3 .. 2048" in L.gsb_last_error() or b"bad arguments" in L.gsb_last_error()
     assert L.gsb_eval_crop_polygon(None, 0, fake, 3, 2, 0.0, 1.0, None, None, None, None) == _lib.GSB_OK
-    lo, hi = (C.c_double * 3)(0, 0, 0), (C.c_double * 3)(1, 1, 1)
     ws = L.gsb_eval_voxel_workspace_bytes(10)
     assert ws > 10 * 41 and L.gsb_eval_voxel_workspace_bytes(-1) == 0
-    assert L.gsb_eval_voxel_downsample(fake, 10, lo, hi, 0.0, fake, ws, fake, fake, None) == _lib.GSB_ERR_INVALID
-    assert L.gsb_eval_voxel_downsample(fake, 10, lo, hi, float("nan"), fake, ws, fake, fake, None) == _lib.GSB_ERR_INVALID
-    nan = (C.c_double * 3)(0, float("nan"), 0)
-    assert L.gsb_eval_voxel_downsample(fake, 10, nan, hi, 0.1, fake, ws, fake, fake, None) == _lib.GSB_ERR_INVALID
-    big = (C.c_double * 3)(1e3, 0, 0)
-    assert L.gsb_eval_voxel_downsample(fake, 10, lo, big, 1e-7, fake, ws, fake, fake, None) == _lib.GSB_ERR_INVALID
-    assert b"too small" in L.gsb_last_error()
-    huge = (C.c_double * 3)(2e9, 2e9, 2e9)
-    assert L.gsb_eval_voxel_downsample(fake, 10, lo, huge, 1.0, fake, ws, fake, fake, None) == _lib.GSB_ERR_INVALID
-    assert b"63 bits" in L.gsb_last_error()
-    assert L.gsb_eval_voxel_downsample(fake, 10, lo, hi, 0.1, fake, ws - 1, fake, fake, None) == _lib.GSB_ERR_WORKSPACE
     g = _lib.GsbPointGrid((C.c_double * 3)(0, 0, 0), 1.0, (C.c_int32 * 3)(1, 1, 1), 256, 1, 256, 256)
     for r in (0.0, -1.0, float("inf"), float("nan")):
         assert L.gsb_eval_icp_correspond(C.byref(g), fake, 10, r, fake, fake, None) == _lib.GSB_ERR_INVALID

@@ -264,7 +264,7 @@ def crossing_float(pu_v, a, b):
 
 # ----------------------------------------------------------------------------------------------------- voxel grid
 def voxel_layout(points, vs):
-    """gsb_eval_voxel_downsample's host arithmetic restated: (lo, span, extents, bits per axis)."""
+    """gsb_pcd_voxel_downsample's host arithmetic restated: (lo, span, extents, bits per axis)."""
     p = np.asarray(points, np.float64)
     mn, mx = p.min(0), p.max(0)
     lo = mn - vs * 0.5
