@@ -128,6 +128,8 @@ SIGNATURES = {
     "gsb_pcd_statistical_outliers": (C.c_int, [C.POINTER(GsbPointGrid), C.c_int32, C.c_double, _vp, C.c_size_t, _vp, _vp, _vp,
                                                _vp]),
     "gsb_pcd_radius_outliers": (C.c_int, [C.POINTER(GsbPointGrid), C.c_int64, C.c_double, _vp, _vp]),
+    "gsb_pcd_dbscan_workspace_bytes": (C.c_size_t, [C.c_int64]),
+    "gsb_pcd_dbscan": (C.c_int, [C.POINTER(GsbPointGrid), C.c_double, C.c_int64, _vp, C.c_size_t, _vp, _vp, _vp]),
     "gsb_eval_transform_points": (C.c_int, [_vp, C.c_int64, C.POINTER(C.c_double), _vp, _vp]),
     "gsb_eval_crop_polygon": (C.c_int, [_vp, C.c_int64, _vp, C.c_int32, C.c_int32, C.c_double, C.c_double, _vp, _vp, _vp, _vp]),
     "gsb_eval_voxel_workspace_bytes": (C.c_size_t, [C.c_int64]),

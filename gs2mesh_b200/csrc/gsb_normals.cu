@@ -1,14 +1,18 @@
 // Exact k nearest neighbours on the shared point grid, and Open3D 0.17's PointCloud::EstimateNormals with
 // KDTreeSearchParamKNN(k) and fast_normal_computation (ComputeCovariance, FastEigen3x3) for a cloud without normals: the
 // Tanks and Temples toolbox's estimate_normals (evaluation.py:60-84).  Open3D 0.17's PointCloud::RemoveStatisticalOutliers
-// and RemoveRadiusOutliers on the same grid (DESIGN.md section 7, "Point-cloud cleaning and downsampling").
+// and RemoveRadiusOutliers on the same grid (DESIGN.md section 7, "Point-cloud cleaning and downsampling"), and its
+// PointCloud::ClusterDBSCAN (DESIGN.md section 7, "Density clustering").
 //
 // Every fp64 operation carries an explicit rounding intrinsic, so nvcc cannot contract a multiply-add into an FMA, and
 // acos / cos are fdlibm's algorithms in those operations rather than the device's libm: tests/normals_oracle.py restates
 // the same operations in numpy and the results compare bit for bit.
+#include <cub/cub.cuh>
+
 #include "gs2mesh_b200.h"
 #include "gsb_common.h"
 #include "gsb_grid.cuh"
+#include "gsb_union_find.cuh"
 
 namespace gsb {
 namespace {
@@ -379,6 +383,97 @@ __global__ void __launch_bounds__(256) radius_outlier_kernel(const GsbPointGrid 
   keep[t] = count > nb_points;
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// ClusterDBSCAN.  core[i] = count_i >= min_points is radius_outlier_kernel with nb_points = min_points - 1 (-1 for
+// min_points = 0 marks every point core).  Core points joined by a pair at d2 < r2 form components; each component's
+// union-find root is its smallest index, so an exclusive scan of the root flags numbers the components by their
+// smallest core index, as Open3D's ascending loop does.  A non-core point takes the smallest root among the core points
+// within eps, which is the smallest component number; none gives -1.
+// ---------------------------------------------------------------------------------------------------------------------
+__device__ __forceinline__ bool finite3(const double* p) { return isfinite(p[0]) && isfinite(p[1]) && isfinite(p[2]); }
+
+// parent[i] = i; a point with a non-finite coordinate is never core (radius_outlier_kernel marks it core for
+// min_points = 0, its count 0 being > -1), so the later passes need not test finiteness of core points.
+__global__ void __launch_bounds__(256) dbscan_init_kernel(const GsbPointGrid g, uint8_t* __restrict__ core,
+                                                          int* __restrict__ parent) {
+  const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= g.n_points) return;
+  parent[t] = (int)t;
+  if (!finite3(g.points + 3 * t)) core[t] = 0;
+}
+
+// One thread per core point i: every core q < i within eps is united with i, so each core-core pair is handled once.
+__global__ void __launch_bounds__(256) dbscan_link_kernel(const GsbPointGrid g, double r2, const uint8_t* __restrict__ core,
+                                                          int* parent) {
+  const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= g.n_points || !core[t]) return;
+  const double x = g.points[3 * t], y = g.points[3 * t + 1], z = g.points[3 * t + 2];
+  visit_27_cells(g, x, y, z, [&](long long q) {
+    if (q < t && core[q] && sq_dist(x, y, z, g.points + 3 * q) < r2) uf_union(parent, (int)t, (int)q);
+    return true;
+  });
+}
+
+// parent[i] = the root of core point i; head[i] = 1 for the roots (core points only)
+__global__ void __launch_bounds__(256) dbscan_compress_kernel(const uint8_t* __restrict__ core, long long n, int* parent,
+                                                              int* __restrict__ head) {
+  const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= n) return;
+  int r = (int)t;
+  if (core[t]) {
+    for (int p = uf_load(parent, r); p != r; p = uf_load(parent, r)) r = p;
+    ParentRef(parent[t]).store(r, cuda::memory_order_relaxed);
+  }
+  head[t] = core[t] && r == (int)t;
+}
+
+// labels[i] = ordinal of i's root (core), of the smallest root among the core points within eps (non-core), or -1; the
+// last thread writes the number of clusters.
+__global__ void __launch_bounds__(256) dbscan_label_kernel(const GsbPointGrid g, double r2, const uint8_t* __restrict__ core,
+                                                           const int* __restrict__ parent, const int* __restrict__ head,
+                                                           const int* __restrict__ ordinal, int32_t* __restrict__ labels,
+                                                           int32_t* __restrict__ n_clusters) {
+  const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= g.n_points) return;
+  const double* p = g.points + 3 * t;
+  int root = -1;
+  if (core[t]) {
+    root = parent[t];
+  } else if (finite3(p)) {
+    const double x = p[0], y = p[1], z = p[2];
+    visit_27_cells(g, x, y, z, [&](long long q) {
+      if (core[q] && (root < 0 || parent[q] < root) && sq_dist(x, y, z, g.points + 3 * q) < r2) root = parent[q];
+      return true;
+    });
+  }
+  labels[t] = root < 0 ? -1 : ordinal[root];
+  if (t == g.n_points - 1) *n_clusters = ordinal[t] + head[t];
+}
+
+// Workspace of gsb_pcd_dbscan; with a NULL base only `total` is meaningful.
+struct DbscanWork {
+  uint8_t* core;  // [n]
+  int* parent;    // [n]
+  int* head;      // [n]
+  int* ordinal;   // [n]
+  void* tmp;
+  size_t tmp_bytes, total;
+};
+
+DbscanWork carve_dbscan(void* base, long long n) {
+  Carver c(base);
+  DbscanWork w;
+  w.core = c.take<uint8_t>((size_t)n);
+  w.parent = c.take<int>((size_t)n);
+  w.head = c.take<int>((size_t)n);
+  w.ordinal = c.take<int>((size_t)n);
+  w.tmp_bytes = 0;
+  cub::DeviceScan::ExclusiveSum(nullptr, w.tmp_bytes, (int*)nullptr, (int*)nullptr, n);
+  w.tmp = c.take<char>(w.tmp_bytes);
+  w.total = c.total();
+  return w;
+}
+
 }  // namespace
 }  // namespace gsb
 
@@ -447,6 +542,37 @@ int gsb_pcd_radius_outliers(const GsbPointGrid* grid, int64_t nb_points, double 
   radius_outlier_kernel<<<blocks_for(grid->n_points), 256, 0, stream>>>(*grid, nb_points, radius * radius, keep);
   count_launch();
   return check_launch("radius_outlier_kernel", stream, false);
+}
+
+size_t gsb_pcd_dbscan_workspace_bytes(int64_t n_points) {
+  if (n_points <= 0 || n_points > 2147483647) return 0;
+  return carve_dbscan(nullptr, n_points).total;
+}
+
+int gsb_pcd_dbscan(const GsbPointGrid* grid, double eps, int64_t min_points, void* workspace, size_t workspace_bytes,
+                   int32_t* labels, int32_t* n_clusters, void* stream_v) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
+  if (!grid_ok(grid) || grid->n_points > 2147483647 || !(eps >= 0.0) || !(eps < INFINITY) || min_points < 0 ||
+      !(grid->cell >= eps * 1.0000001) || (grid->n_points && (!workspace || !labels || !n_clusters)))
+    return fail(GSB_ERR_INVALID,
+                "pcd_dbscan: bad arguments (a finite eps >= 0, min_points >= 0, the grid cell above eps, at most 2^31 - 1 "
+                "points)");
+  const long long n = grid->n_points;
+  if (n == 0) return GSB_OK;
+  const size_t need = gsb_pcd_dbscan_workspace_bytes(n);
+  if (workspace_bytes < need) return fail(GSB_ERR_WORKSPACE, "pcd_dbscan: workspace %zu < %zu bytes", workspace_bytes, need);
+  const DbscanWork w = carve_dbscan(workspace, n);
+  const double r2 = eps * eps;
+  radius_outlier_kernel<<<blocks_for(n), 256, 0, stream>>>(*grid, min_points - 1, r2, w.core);
+  dbscan_init_kernel<<<blocks_for(n), 256, 0, stream>>>(*grid, w.core, w.parent);
+  dbscan_link_kernel<<<blocks_for(n), 256, 0, stream>>>(*grid, r2, w.core, w.parent);
+  dbscan_compress_kernel<<<blocks_for(n), 256, 0, stream>>>(w.core, n, w.parent, w.head);
+  count_launch(4);
+  size_t tmp_bytes = w.tmp_bytes;
+  GSB_CUDA_OK(cub::DeviceScan::ExclusiveSum(w.tmp, tmp_bytes, w.head, w.ordinal, n, stream));
+  dbscan_label_kernel<<<blocks_for(n), 256, 0, stream>>>(*grid, r2, w.core, w.parent, w.head, w.ordinal, labels, n_clusters);
+  count_launch();
+  return check_launch("pcd_dbscan", stream, false);
 }
 
 }  // extern "C"

@@ -1,5 +1,5 @@
 // Lock-free union-find, the undirected edge key and its sort width, shared by the mesh cluster kernels (gsb_mesh.cu)
-// and the topology queries (gsb_topology.cu).
+// and the topology queries (gsb_topology.cu); the union-find also joins DBSCAN's core points (gsb_normals.cu).
 //
 // Union-find over int ids in the style of ECL-CC: a larger root is always hooked under a smaller one with atomicCAS, so
 // parent[x] <= x holds at every moment and the surviving root of a set is its smallest id.  Parents are read with

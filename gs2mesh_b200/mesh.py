@@ -10,9 +10,9 @@ both give the same labels, counts and cleaned mesh.  Vertex-clustering simplific
 simplify_vertex_clustering) and the smoothing and sharpening filters (filter_smooth_simple / _laplacian / _taubin,
 filter_sharpen) run on the GPU, and so do the topology queries (manifoldness, orientability, self-intersection,
 watertightness, Euler characteristic, surface area and volume).  The extracted PointCloud is cleaned and thinned on the GPU
-too (gs2mesh_b200/pointcloud.py): remove_statistical_outlier, remove_radius_outlier, select_by_index, voxel_down_sample
-with colours and normals, uniform_down_sample, compute_nearest_neighbor_distance and compute_point_cloud_distance.  PLY
-writing stays on the host like in the reference.
+too (gs2mesh_b200/pointcloud.py): remove_statistical_outlier, remove_radius_outlier, cluster_dbscan, select_by_index,
+voxel_down_sample with colours and normals, uniform_down_sample, compute_nearest_neighbor_distance and
+compute_point_cloud_distance.  PLY writing stays on the host like in the reference.
 """
 from __future__ import annotations
 
@@ -531,12 +531,12 @@ class PointCloud:
         self.points = (self.points - c) * float(scale) + c
         return self
 
-    # -- PointCloud::RemoveStatisticalOutliers / RemoveRadiusOutliers / SelectByIndex / VoxelDownSample /
+    # -- PointCloud::RemoveStatisticalOutliers / RemoveRadiusOutliers / ClusterDBSCAN / SelectByIndex / VoxelDownSample /
     # UniformDownSample / ComputeNearestNeighborDistance / ComputePointCloudDistance (DESIGN.md section 7, "Point-cloud
-    # cleaning and downsampling"; gs2mesh_b200/pointcloud.py).  Each runs on `self.device` (the current CUDA device for a
-    # cloud built from host arrays), returns a new cloud of the same class holding host arrays with that device set, or
-    # host values, and leaves the cloud unchanged; colours and normals travel with their points.  ValueError for
-    # non-finite points, a colour or normal array without one row per point, or 2^31 points or more.
+    # cleaning and downsampling" and "Density clustering"; gs2mesh_b200/pointcloud.py).  Each runs on `self.device` (the
+    # current CUDA device for a cloud built from host arrays), returns a new cloud of the same class holding host arrays
+    # with that device set, or host values, and leaves the cloud unchanged; colours and normals travel with their points.
+    # ValueError for non-finite points, a colour or normal array without one row per point, or 2^31 points or more.
     def remove_statistical_outlier(self, nb_neighbors, std_ratio, print_progress=False):
         """(cloud, int64 indices ascending): keeps point i iff its mean distance m_i to its nb_neighbors nearest points
         (itself included) satisfies 0 < m_i < mean + std_ratio * std of the positive m_i over the cloud's n points."""
@@ -546,6 +546,11 @@ class PointCloud:
         """(cloud, int64 indices ascending): keeps point i iff more than nb_points points (itself included) lie at squared
         distance strictly below radius * radius."""
         return _pcd.remove_radius_outlier(self, nb_points, radius)
+
+    def cluster_dbscan(self, eps, min_points, print_progress=False):
+        """int32 numpy (n,): DBSCAN cluster labels, numbered by each cluster's smallest core point index, -1 for noise
+        (DESIGN.md section 7, "Density clustering")."""
+        return _pcd.cluster_dbscan(self, eps, min_points)
 
     def select_by_index(self, indices, invert=False):
         """The points at `indices` (or, with invert, the others) in ascending index order, each once."""

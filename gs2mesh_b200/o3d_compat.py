@@ -39,6 +39,7 @@ and the cleaning and thinning of the extracted cloud (each returns a new cloud; 
     clean, ind = pcd.remove_statistical_outlier(nb_neighbors=20, std_ratio=2.0)
     clean, ind = pcd.remove_radius_outlier(nb_points=16, radius=0.05)
     thin = clean.voxel_down_sample(voxel_size=0.01)          # colours and normals averaged
+    labels = pcd.cluster_dbscan(eps=0.02, min_points=10)    # int32 numpy labels, -1 for noise
     # also select_by_index, uniform_down_sample, compute_nearest_neighbor_distance, compute_point_cloud_distance
 
 Differences from Open3D, by construction: the volume lives in GPU memory (an unbounded, hashed set of 16^3 bricks on

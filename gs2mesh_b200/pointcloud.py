@@ -1,11 +1,13 @@
 """Point-cloud cleaning and downsampling on the GPU: Open3D 0.17's PointCloud.remove_statistical_outlier,
-remove_radius_outlier, select_by_index, voxel_down_sample (with colours and normals), uniform_down_sample,
-compute_nearest_neighbor_distance and compute_point_cloud_distance, for gs2mesh_b200.mesh.PointCloud (whose methods call
-these functions).  DESIGN.md section 7, "Point-cloud cleaning and downsampling", restates each operation and its doubt
-points; tests/pcd_oracle.py restates them in numpy.
+remove_radius_outlier, cluster_dbscan, select_by_index, voxel_down_sample (with colours and normals),
+uniform_down_sample, compute_nearest_neighbor_distance and compute_point_cloud_distance, for
+gs2mesh_b200.mesh.PointCloud (whose methods call these functions).  DESIGN.md section 7, "Point-cloud cleaning and
+downsampling" and "Density clustering", restates each operation and its doubt points; tests/pcd_oracle.py and
+tests/dbscan_oracle.py restate them in numpy.
 
 The neighbour searches run on the shared point grid (evaluate.PointGrid): gsb_pcd_statistical_outliers and
-gsb_pcd_radius_outliers of include/gs2mesh_b200.h for the outlier tests, gsb_pcd_voxel_downsample for the voxel means.
+gsb_pcd_radius_outliers of include/gs2mesh_b200.h for the outlier tests, gsb_pcd_dbscan for the clusters,
+gsb_pcd_voxel_downsample for the voxel means.
 Index selection and the final compaction are torch gathers on the device.  Every function runs on the cloud's device
 (the current CUDA device for a cloud built from host arrays), returns a new cloud of the caller's class holding host
 arrays with that device set, and leaves the cloud it was given unchanged.
@@ -137,6 +139,42 @@ def remove_radius_outlier(pcd, nb_points, radius, print_progress=False):
     dev = keep.device
     with torch.cuda.device(dev):
         return _select(pcd, dev, keep), keep.nonzero()[:, 0].cpu().numpy()
+
+
+def dbscan(pcd, eps, min_points):
+    """(labels device int32 [n], n_clusters device int32 [1]) of gsb_pcd_dbscan, None for an empty cloud; argument
+    errors as cluster_dbscan."""
+    e = float(eps)
+    m = _size_t(min_points, "min_points")
+    if not (math.isfinite(e) and e >= 0.0):
+        raise ValueError(f"cluster_dbscan: eps must be finite and >= 0, got {e}")
+    n = _check(pcd, "cluster_dbscan")
+    if n == 0:
+        return None
+    dev = _lib.device(pcd.device)
+    L = _lib.lib()
+    with torch.cuda.device(dev):
+        grid = PointGrid(torch.as_tensor(pcd.points).to(dev), radius=e)
+        work = torch.empty(int(L.gsb_pcd_dbscan_workspace_bytes(n)), dtype=torch.uint8, device=dev)
+        labels = torch.empty(n, dtype=torch.int32, device=dev)
+        n_clusters = torch.empty(1, dtype=torch.int32, device=dev)
+        # min_points past n + 1 makes no point core, like n + 1 does
+        _lib.check(L.gsb_pcd_dbscan(C.byref(grid.desc), e, min(m, n + 1), ptr(work), work.numel(), ptr(labels),
+                                    ptr(n_clusters), _lib.stream(dev)), invalid_is_value_error=True)
+    return labels, n_clusters
+
+
+def cluster_dbscan(pcd, eps, min_points, print_progress=False):
+    """int32 numpy [n]: Open3D's DBSCAN labels.  Point i is core iff at least min_points points (itself included) lie at
+    squared distance strictly below eps * eps; core points joined by such pairs form clusters, numbered 0, 1, ... by
+    their smallest core index; a non-core point within eps of a core point takes the smallest number among those
+    points' clusters, any other point -1.  TypeError for a negative or non-integer min_points, ValueError for a negative
+    or non-finite eps."""
+    r = dbscan(pcd, eps, min_points)
+    if r is None:
+        return np.zeros(0, np.int32)
+    with torch.cuda.device(r[0].device):
+        return r[0].cpu().numpy()
 
 
 def _empty_like(pcd):

@@ -597,6 +597,18 @@ size_t gsb_pcd_statistical_workspace_bytes(int64_t n_points);
 int gsb_pcd_statistical_outliers(const GsbPointGrid* grid, int32_t k, double std_ratio, void* workspace,
                                  size_t workspace_bytes, double* mean_dist, uint8_t* keep, double* stats, void* stream);
 int gsb_pcd_radius_outliers(const GsbPointGrid* grid, int64_t nb_points, double radius, uint8_t* keep, void* stream);
+/* Density clustering: Open3D 0.17's PointCloud::ClusterDBSCAN(eps, min_points) over the grid's points (gsb_normals.cu;
+ * DESIGN.md section 7, "Density clustering"; restated in tests/dbscan_oracle.py).  Same contract as the cleaning block
+ * above (refusals before anything is enqueued, no allocation, no host sync, the same bytes on every run).  Point i is
+ * core iff count_i >= min_points, count_i = #{j : ((dx*dx)+dy*dy)+dz*dz < eps*eps}, i included (strict, as
+ * gsb_pcd_radius_outliers).  Core points joined by such pairs form components, numbered 0, 1, ... by their smallest
+ * core index; labels[i] (device int32 [n]) = the component of a core point, the smallest component among the core points
+ * within eps of a non-core point, or -1 (noise, and every point with a non-finite coordinate).  n_clusters: device int32,
+ * the number of components.  eps finite and >= 0, min_points >= 0, the grid cell at least eps * 1.0000001, n < 2^31.
+ * One caller workspace of gsb_pcd_dbscan_workspace_bytes(n) (0 for invalid sizes), else GSB_ERR_WORKSPACE. */
+size_t gsb_pcd_dbscan_workspace_bytes(int64_t n_points);
+int gsb_pcd_dbscan(const GsbPointGrid* grid, double eps, int64_t min_points, void* workspace, size_t workspace_bytes,
+                   int32_t* labels, int32_t* n_clusters, void* stream);
 
 /* Tanks and Temples evaluation (evaluation/TNT/eval_code/python_toolbox/evaluation), restating Open3D 0.17's
  * PointCloud::Transform, SelectionPolygonVolume::CropInPolygon, VoxelDownSample and RegistrationICP with
